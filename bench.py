@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline measurement of the wavefront hot path (contract in the task brief).
+"""bench.py -- headline measurement of the wavefront hot path.
 
 step      = one full-field CVP plan (CVPMeshPlanner::waveFrontPropagation, no goal cutoff) per GPU
             on the 5M-vertex synthetic terrain mesh (2240 x 2240, SURVEY.md 8d); with N GPUs every
@@ -9,7 +9,8 @@ value     = settled vertices of all ranks / device time, inputs already resident
 e2e       = same plan through the C ABI with HOST buffers: vertex_costs + edge_weights copied H2D
             (mnb_set_costs) and potential/pred/direction/cutting_face copied D2H every step.
 roofline  = dominant kernel k_cvp: algorithmic bytes (208 B / settled vertex, SURVEY.md 8d) / its
-            CUDA-event duration, against the measured HBM copy bandwidth (MEASURED_PEAKS.json).
+            CUDA-event duration, against the measured HBM copy bandwidth (MEASURED_PEAKS.json) if present, else the
+            H100 SXM data sheet's 3.35 TB/s.
 cpu_baseline = the oracle (reference algorithm restated, 1 thread, as the reference is per plan), rebuilt on the box
             with -O3 -march=native (BASELINE.md section 2).
 config.parity    = the potentials / predecessors of the TIMED 5M plan against the oracle's plan on the same input
@@ -18,9 +19,10 @@ config.config3   = BASELINE config 3 as a plan: fused layers -> Max combination 
                    1000 obstacle discs) -> vertex_costs -> computeEdgeWeights(edge_cost_factor 1) -> CVP with
                    cost_limit 1 on those costs, timed, with its own parity block.
 config.batched   = BASELINE config 4 (1024 goals, 1M-vertex terrain, goal k -> rank k mod N, potentials all-gathered):
-                   plans/s, HBM fraction and 8 sampled fields against the oracle -- inside `config` because the driver
-                   keeps that object for every N.
+                   plans/s, HBM fraction and 8 sampled fields against the oracle -- inside `config` so that it is kept
+                   with the line of every N.
 --impl reference: the oracle on the host cores, one independent plan per thread.
+--dump-outputs DIR: the arrays of the last timed plan as DIR/<name>.npy (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -45,7 +47,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -72,6 +74,7 @@ class ClockSampler:
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
+        self.proc.wait()
         sm, mx, reasons = [], [], set()
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
@@ -86,15 +89,6 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
-
-
-def ncu_traffic(workload):
-    """dram bytes (read + write) per launch of the dominant kernel from the committed `ncu --set full` capture"""
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")) as f:
-            return json.load(f).get(workload)
-    except Exception:
-        return None
 
 
 def build_workload(n):
@@ -133,12 +127,33 @@ def parity_block(got_dist, got_pred, ref, got_cut=None):
     return out
 
 
+DUMP_BUDGET = 64 * 1000 * 1000      # bytes, .npy headers included
+
+
+def dump_outputs(out_dir, dist, pred, direction, cut):
+    """The arrays a caller of the timed plan receives (potential, predecessor, direction, cutting face), one .npy each:
+    floats as float32, indices as float64 (exact).  Above DUMP_BUDGET bytes every array is cut to the same fixed, seeded
+    sample of vertices, whose ids are written as vertex_index.npy, so that two builds can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"potential": dist.astype(np.float32), "predecessor": pred.astype(np.float64),
+              "direction": direction.astype(np.float32), "cutting_face": cut.astype(np.float64)}
+    V = dist.size
+    per_vertex = sum(a.itemsize for a in arrays.values())
+    if V * per_vertex > DUMP_BUDGET:
+        keep = (DUMP_BUDGET - 4096) // (per_vertex + 8)
+        idx = np.sort(np.random.default_rng(0).choice(V, size=keep, replace=False))
+        arrays = {k: a[idx] for k, a in arrays.items()}
+        arrays["vertex_index"] = idx.astype(np.float64)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
+
+
 CONFIG_KEYS = ("workload", "vertices", "faces", "edges", "plans_per_step_per_gpu", "sharding", "l2", "parity", "config3", "batched")
 
 
 def run_reference(args):
     """--impl reference: the reference's CPU algorithm (oracle port; lvr2 / ROS 2 cannot be installed offline)
-    on the host cores, on the SAME workload as the B200 arm: one full-field CVP plan on the 5M-vertex terrain per
+    on the host cores, on the SAME workload as the GPU arm: one full-field CVP plan on the 5M-vertex terrain per
     step.  The reference plans one query on one thread (MeshPlannerExecution::makePlan runs the heap loop on the
     planner thread, mesh_planner_execution.cpp:55-66), so a single plan uses 1 core; the batched sub-result uses
     one independent plan per host thread on all cores (BASELINE.md section 2)."""
@@ -225,6 +240,8 @@ def main():
     ap.add_argument("--no-config3", action="store_true")
     ap.add_argument("--no-other-kernels", action="store_true")
     ap.add_argument("--submesh-from", type=int, default=3000, help="grid side from which the 1M sub-mesh parity spot check runs (config 5)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed plan returned (rank 0) as DIR/<name>.npy, at most 64 MB in all")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)
@@ -235,7 +252,7 @@ def main():
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the product has no CPU path")
+        raise SystemExit("bench.py needs an H100: the product has no CPU path")
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
@@ -257,7 +274,7 @@ def main():
     d_dir = torch.empty(V, dtype=torch.float32, device=dev)
     d_cut = torch.empty(V, dtype=torch.int32, device=dev)
     gathered = [torch.empty(V, dtype=torch.float32, device=dev) for _ in range(world)] if world > 1 else None
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 256 MB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 256 MB > the H100's 50 MB L2
 
     def step_resident():
         flush.zero_()                                   # L2 flush between timed iterations (untimed kernels are tiny)
@@ -296,8 +313,10 @@ def main():
         dt_max = dt; total_settled = float(settled)
     clocks = sampler.stop(local)
     value = total_settled * args.steps / dt_max
-    # the result of the LAST TIMED plan, for the parity block (rank 0)
+    # the result of the LAST TIMED plan, for the parity block and --dump-outputs (rank 0)
     h_timed = None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, d_dist.cpu().numpy(), d_pred.cpu().numpy().view(np.uint32), d_dir.cpu().numpy(), d_cut.cpu().numpy())
     if rank == 0 and not args.no_cpu_baseline:
         h_timed = {"dist": d_dist.cpu().numpy(), "pred": d_pred.cpu().numpy().view(np.uint32), "cut": d_cut.cpu().numpy()}
 
@@ -672,7 +691,6 @@ def main():
         hbm, which = peaks()
         k_ms = float(np.mean(kernel_ms))
         achieved = CVP_BYTES_PER_VERTEX * settled / (k_ms * 1e-3) / 1e9
-        traffic = ncu_traffic(f"cvp_full_field_terrain_{n}x{n}")
         config = {"workload": f"cvp_full_field_terrain_{n}x{n}", "vertices": V, "faces": mm.F, "edges": E,
                   "plans_per_step_per_gpu": 1, "sharding": "one goal per GPU (distinct goals within 2% of the map centre: same wave depth on every rank), potentials all-gathered (NCCL)" if world > 1 else "single GPU",
                   "l2": "256 MB buffer rewritten between timed iterations; working set (>500 MB) exceeds L2",
@@ -686,8 +704,7 @@ def main():
                     "d2h_bytes_per_step": int(16 * V), "steps": e2e_steps},
             "gpu_launches": int(args.steps * st["kernel_launches"]),
             "roofline": {"bound": "hbm", "kernel": "k_cvp_grid", "achieved": achieved, "peak": hbm, "unit": "GB/s",
-                         "frac": achieved / hbm, "traffic": traffic["bytes"] if isinstance(traffic, dict) else traffic,
-                         "traffic_source": traffic.get("source") if isinstance(traffic, dict) else None, "peak_source": which,
+                         "frac": achieved / hbm, "traffic": None, "peak_source": which,
                          "kernel_ms": k_ms, "rounds": int(st["rounds"]), "recomputes_per_vertex": st["recomputes"] / V,
                          "deep_cascade_labels": int(st.get("deep_labels", 0)),
                          "batched_plans_per_s": batched.get("plans_per_s") if batched else None,

@@ -1,7 +1,7 @@
 /*
  * meshnav_b200.h -- C ABI of libmeshnav_b200.so
  *
- * B200-native (sm_100a CUDA) replacement for the wavefront hot path of
+ * H100-native (sm_90a CUDA) replacement for the wavefront hot path of
  * naturerobots/mesh_navigation.  Plain pointers and sizes only; no C++ / torch
  * types cross this boundary.  Every entry point names the reference interface
  * it stands in for (paths relative to the reference repo).
@@ -22,7 +22,7 @@
  *     point that may be called concurrently from another thread
  *     (reference: CVPMeshPlanner::cancel, cvp_mesh_planner.cpp:142-146).
  *   - there is NO CPU fallback: every compute entry point fails with
- *     MNB_E_CUDA if no sm_100 device is usable.
+ *     MNB_E_CUDA if no sm_90 device is usable.
  */
 #ifndef MESHNAV_B200_H
 #define MESHNAV_B200_H

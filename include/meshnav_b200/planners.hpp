@@ -66,7 +66,7 @@ enum : uint32_t { SUCCESS = 0, CANCELED = 51, INVALID_START = 52, INVALID_GOAL =
 class MeshMap {
  public:
   MeshMap(const std::vector<float>& pos, const std::vector<uint32_t>& faces, int device = 0) : pos_(pos), faces_(faces) {
-    if (mnb_create(device, &ctx_) != MNB_OK) throw std::runtime_error("meshnav_b200: no usable sm_100 device (no CPU fallback)");
+    if (mnb_create(device, &ctx_) != MNB_OK) throw std::runtime_error("meshnav_b200: no usable sm_90 device (no CPU fallback)");
     if (mnb_set_mesh(ctx_, (uint32_t)(pos.size() / 3), (uint32_t)(faces.size() / 3), pos.data(), faces.data(), nullptr, 0) != MNB_OK)
       throw std::runtime_error(mnb_last_error(ctx_));
     vertex_costs_.assign(numVertices(), 0.0f);

@@ -1,6 +1,6 @@
 """ctypes binding of libmeshnav_b200.so (include/meshnav_b200.h).
 
-There is no fallback: if the shared library is missing or no sm_100 device is
+There is no fallback: if the shared library is missing or no sm_90 device is
 usable, importing works but every compute call raises.
 """
 from __future__ import annotations
@@ -69,7 +69,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(f"{LIB_PATH} is missing: build it with __graft_entry__.build() "
-                           "(nvcc, sm_100a). There is no CPU fallback.")
+                           "(nvcc, sm_90a). There is no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp, i32, u32, i64, dbl, f32 = C.c_void_p, C.c_int32, C.c_uint32, C.c_int64, C.c_double, C.c_float
     L.mnb_create.restype = i32; L.mnb_create.argtypes = [i32, C.POINTER(vp)]

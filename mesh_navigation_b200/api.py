@@ -38,7 +38,7 @@ class MeshMap:
         self._ctx = C.c_void_p()
         rc = self.L.mnb_create(device, C.byref(self._ctx))
         if rc != 0:
-            raise MeshNavError(f"mnb_create failed ({rc}): no usable sm_100 CUDA device; there is no CPU fallback")
+            raise MeshNavError(f"mnb_create failed ({rc}): no usable sm_90 CUDA device; there is no CPU fallback")
         self.pos = np.ascontiguousarray(pos, dtype=np.float32).reshape(-1, 3)
         self.faces = np.ascontiguousarray(faces, dtype=np.uint32).reshape(-1, 3)
         e = None if edges is None else np.ascontiguousarray(edges, dtype=np.uint32).reshape(-1, 2)

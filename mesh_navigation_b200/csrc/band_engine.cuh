@@ -1,4 +1,4 @@
-// Sliding-band pull wavefront engine (sm_100a).
+// Sliding-band pull wavefront engine (sm_90a).
 //
 // What it replaces: the heap loops of the reference
 //   CVPMeshPlanner::waveFrontPropagation   cvp_mesh_planner.cpp:747-886
@@ -7,7 +7,7 @@
 // which pop one vertex at a time from lvr2::Meap and push updates to the free
 // vertex of every incident face (edge) that has all its other vertices fixed.
 //
-// B200 formulation (not a translation of the heap):
+// GPU formulation (not a translation of the heap):
 //   * every vertex carries one 16-byte word  {d : potential, a1, a2, a3 : pop time}.
 //     The pop time is the moment the sequential algorithm would have popped the
 //     vertex, as a monotonic stack of water levels (problems.cuh); for causal
@@ -27,7 +27,7 @@
 //     {1,2,4,8,16}); the barrier is the hardware cluster barrier (or
 //     __syncthreads for CS==1), not a grid-wide sync, so a round costs ~1 us
 //     instead of a kernel launch.  Batches run one wavefront per cluster on all
-//     148 SMs; CS==0 selects a cooperative whole-grid group (used by the
+//     SMs; CS==0 selects a cooperative whole-grid group (used by the
 //     multi-source inflation wave which has few, very wide rounds).
 //   * the next round's candidate list is staged in shared memory per CTA and
 //     flushed with one global atomic per CTA per round.
@@ -80,7 +80,7 @@ struct TimeAlg {
   // levels 2.. tie on the key of level 2 (rare: same cascade, bit-identical keys or the same sub-trigger)
   // (the out-of-line helpers take pop times BY VALUE: a by-reference argument of a __noinline__ callee forces the caller's
   // variable into local memory for its whole lifetime -- labels a, b, T and tc of the hot path were stored to the stack on
-  // every evaluation while these took references, profiles/r02o)
+  // every evaluation while these took references)
   __device__ __noinline__ bool less_tail(const EvTime x, const EvTime y) const {
     const uint32_t i2x = id2_of(x), i2y = id2_of(y);
     if (i2x != i2y) return i2x < i2y;

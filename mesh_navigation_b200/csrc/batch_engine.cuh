@@ -3,10 +3,8 @@
 // Same algorithm, same label format and bit-identical results as run_band_rounds_sub8 (band_engine.cuh); what differs is
 // what the hot loop carries.  The generic loop serves single plans (goal cutoff + re-queueing, in-round sweeps, the
 // clean-candidate skip, robot bookkeeping) and holds the whole problem object live: at the 64 registers a 2-CTA/SM batch
-// kernel may use it spilled -- ncu on 296 x 1M-vertex plans (profiles/r02_ncu_batch.md, r02a_k_cvp_batch_legacy_*): 11.7 % of all executed
-// instructions were LDL/STL, the local-memory footprint (240 MB) did not fit the L2 and local traffic was 3x the global
-// traffic, 559 warp-instructions per 4-candidate iteration at 34 % issue utilisation, everything waiting on the long
-// scoreboard.  A batch needs none of the extras:
+// kernel may use it spilled: a large share of the executed instructions become local loads and stores, and with
+// hundreds of wavefronts in flight the local-memory footprint does not fit the L2.  A batch needs none of the extras:
 //   * fast path (98 % of the evaluations): every source label is plain (one level), no source can be a seed, the causal
 //     collapse applies -> the new label is min over the causal faces; nothing but the kernel parameters (constant bank)
 //     and five per-wavefront pointers stay live, no problem object, no pop-time algebra;
@@ -414,8 +412,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
             const uint32_t kb = __float_as_uint(fminf(tau, m));
 #ifndef MNB_BATCH_SERIAL_ACTIVATION
             // The activation used to test mark[x] neighbour by neighbour inside the loop that also issues the CAS and the stage
-            // write: twelve dependent L2 round trips for the one evaluation per vertex that activates (11 % of the kernel's
-            // stall samples, profiles/r02_ncu_batch.md).  Now the marks of the whole ring are requested first (no store in
+            // write: twelve dependent L2 round trips for the one evaluation per vertex that activates.  Now the marks of the whole ring are requested first (no store in
             // that loop, so the loads overlap) and only the unmarked, eligible neighbours take the CAS.
             uint32_t todo = 0u;
             if (act_now) {

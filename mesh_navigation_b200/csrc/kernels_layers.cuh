@@ -187,7 +187,7 @@ __device__ __forceinline__ void walk(const LayerKernelArgs& a, uint32_t v, float
 // Variant with the `seen` hash set and the traversal stack in SHARED memory (slot-major, one bank per thread: conflict
 // free) instead of thread-local memory: 1536 resident threads x ~0.9 KB of randomly probed local memory does not fit the
 // L1, so every probe of the local-memory version is an L2 trip.  Same traversal, same visiting order, same sums.
-// Opt-in (MNB_LAYERS_SMEM=1) until it has been timed on a B200.
+// Opt-in (MNB_LAYERS_SMEM=1).
 constexpr int LS_THREADS = 128, LS_STACK = 48;
 template <int WHICH>
 __device__ __forceinline__ void walk_smem(const LayerKernelArgs& a, uint32_t v, float radius, float& zmin, float& zmax,

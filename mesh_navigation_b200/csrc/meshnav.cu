@@ -1,5 +1,5 @@
-// libmeshnav_b200.so -- C ABI (include/meshnav_b200.h) over the sm_100a kernels.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -fmad=false -std=c++17
+// libmeshnav_b200.so -- C ABI (include/meshnav_b200.h) over the sm_90a kernels.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -fmad=false -std=c++17
 //             -Xcompiler -fPIC -shared -o libmeshnav_b200.so meshnav.cu
 #include <cuda_runtime.h>
 
@@ -79,10 +79,10 @@ struct mnb_ctx {
   int grid_blocks_per_sm = 0;
   int infl_skip_clean = 1;     // clean-candidate skip of the inflation wave (MNB_INFL_SKIP=0 turns it off)
   int layers_smem = 5;         // neighbourhood walk of k_layers: 0 thread-local seen-set, 1 shared-memory seen-set, 2-4 prefetching walk (64 / 128 / 32
-                               // threads per CTA), 5-7 the same with the 16-bit seen-set (64 / 128 / 256), 8-9 its low-register builds.  5 M vertices on
-                               // the B200: 8.4 / - / 6.9 / ... / 5.1 ms for modes 0 / 2 / 5.  Chosen per mesh by mnb_set_mesh unless fixed by the caller.
+                               // threads per CTA), 5-7 the same with the 16-bit seen-set (64 / 128 / 256), 8-9 its low-register builds.
+                               // Chosen per mesh by mnb_set_mesh unless fixed by the caller.
   bool layers_explicit = false;
-  int skip_clean = 0;          // clean-candidate stamps of the generic 8-lane CVP loop: measured slower on the B200 (35.8 vs 31.5 ms), its kernel
+  int skip_clean = 0;          // clean-candidate stamps of the generic 8-lane CVP loop: measured slower than without them, its kernel
                                // instantiations are no longer built; the flag only reaches the legacy per-cluster kernel args.  The batch engine
                                // and the inflation wave carry their own (exact) rule.
   int sweeps = -1;             // in-round sweeps of the whole-grid single-plan kernel; -1 = derived from the band width
@@ -182,7 +182,7 @@ int32_t mnb_create(int32_t device, mnb_ctx** out_ctx) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0 || device < 0 || device >= n) return MNB_E_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return MNB_E_CUDA;
-  if (prop.major < 10) return MNB_E_CUDA;   // sm_100a only; no fallback path exists
+  if (prop.major != 9 || prop.minor != 0) return MNB_E_CUDA;   // sm_90a code loads on compute capability 9.0 only; no fallback path exists
   if (cudaSetDevice(device) != cudaSuccess) return MNB_E_CUDA;
   mnb_ctx* c = new mnb_ctx();
   c->device = device; c->sm_count = prop.multiProcessorCount;
@@ -347,7 +347,7 @@ static int32_t install_weights(mnb_ctx* ctx) {
   // scale of the potentials: mean finite edge weight (see mnb_ctx::delta_explicit)
   if (!ctx->d_wsum) CK(dalloc(&ctx->d_wsum, 2));
   CK(cudaMemsetAsync(ctx->d_wsum, 0, 2 * sizeof(double), ctx->stream));
-  MNB_LAUNCH(k_weight_scale, 296, 256, 0, ctx->stream, (const float*)ctx->d_edge_w, ctx->E, ctx->d_wsum);
+  MNB_LAUNCH(k_weight_scale, 2 * ctx->sm_count, 256, 0, ctx->stream, (const float*)ctx->d_edge_w, ctx->E, ctx->d_wsum);
   CK(cudaGetLastError());
   double hs[2] = {0.0, 0.0};
   CK(cudaMemcpyAsync(hs, ctx->d_wsum, sizeof(hs), cudaMemcpyDeviceToHost, ctx->stream));
@@ -357,7 +357,7 @@ static int32_t install_weights(mnb_ctx* ctx) {
     // Single plans: the band should hold about as many candidates as the grid has sweep slots (SM count x Stage::SW_CAP);
     // beyond that the in-round sweeps cannot follow and the band's rows fall out of the L2.  A front is ~3 sqrt(V) vertices
     // long on a compact map and a hop is ~1.35 w deep.  5 M vertices: 20 w / 25 w (the values the kernels were tuned with);
-    // 50 M: 9.6 w -- measured there: CVP 342 -> 232 ms, Dijkstra 178 -> 98 ms against the fixed 20 w / 25 w.
+    // with 132 SMs the band narrows above ~9 M vertices (12 w at 25 M).
     const float slots = (float)ctx->sm_count * (float)Stage::SW_CAP;
     const float hops = slots / (3.0f * sqrtf((float)ctx->V));
     const float k = fmaxf(4.0f, 1.35f * hops);

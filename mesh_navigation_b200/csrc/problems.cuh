@@ -438,7 +438,7 @@ struct CvpEllProblemT : CvpProblem {
       if (j == 0) {
         // (by-reference arguments of a __noinline__ callee live in local memory: keep the address-taken copies inside this
         // rare branch, or every update of cur / tc in the hot path above becomes a local store -- 4.5x the local stores of
-        // the whole kernel when that was overlooked, profiles/r02m)
+        // the whole kernel when that was overlooked)
         const EvTime ot = old_t; float cs; EvTime ts;
         replay_serial(c, band_end, goal, round, ot, cs, ts);
         cur = cs; tc = ts;

@@ -7,9 +7,9 @@ box, gloo in the CPU tests) is plumbing only -- there is no compute step that a 
 tile by tile, hence nothing to fuse.
 
 goal k -> rank k mod N.  By default a rank computes all its goals in ONE batch call (the batch kernel wants as many
-concurrent wavefronts as the GPU holds) followed by one all_gather_into_tensor straight into the final buffer: on the
-8 x B200 box the gather of 1024 x 1M-vertex fields (4 GB per rank) takes ~6 ms over NVSwitch against hundreds of ms of
-compute, so there is nothing worth overlapping.  `chunk > 0` keeps the chunked, overlapped variant (gather of chunk i
+concurrent wavefronts as the GPU holds) followed by one all_gather_into_tensor straight into the final buffer: over
+NVLink / NVSwitch the gather of 1024 x 1M-vertex fields (4 GB per rank) is a small fraction of the batch's compute, so
+there is nothing worth overlapping.  `chunk > 0` keeps the chunked, overlapped variant (gather of chunk i
 runs while chunk i+1 is computed) for maps / goal counts where the fields of a rank do not fit next to the gathered buffer.
 """
 from __future__ import annotations

@@ -1156,7 +1156,7 @@ extern "C" uint32_t orc_inflation_update_set(uint32_t V, const float* new_costs,
 // lvr2::calcNormalClearance (called at clearance_layer.cpp:161).
 //
 // PARITY UNPINNED: the ray/triangle arithmetic lives in lvr2 / Embree (un-vendored, source_dependencies.yaml:4-7) and the
-// reference holds no test or golden vector for it.  Stated here and followed by the B200 kernels:
+// reference holds no test or golden vector for it.  Stated here and followed by the GPU kernels:
 //   * a ray (o, d) meets a triangle (a, b, c) by the two-sided Moeller-Trumbore test in float, evaluated in the order written
 //     in ray_triangle() below, and only inside the triangle's bounding box grown by eps = 1e-5f * max |coordinate| of the map
 //     (box_span(): per-axis slabs; entry tn clamped at 0, exit tf; the hit needs tn <= t <= tf);

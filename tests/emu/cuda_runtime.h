@@ -563,7 +563,7 @@ static inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSu
 static inline cudaError_t cudaGetLastError() { const cudaError_t e = emu::g_last_error; emu::g_last_error = cudaSuccess; return e; }
 static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
-  std::memset(p, 0, sizeof(*p)); p->major = 10; p->minor = 0; p->multiProcessorCount = emu::sm_count();
+  std::memset(p, 0, sizeof(*p)); p->major = 9; p->minor = 0; p->multiProcessorCount = emu::sm_count();
   std::snprintf(p->name, sizeof(p->name), "mnb-emu (CPU interpreter, test only)"); p->totalGlobalMem = emu::ARENA_BYTES;
   return cudaSuccess;
 }

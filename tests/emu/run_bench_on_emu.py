@@ -1,4 +1,4 @@
-"""Dry-run of bench.py's B200 arm on the CPU interpreter of the kernels (tiny sizes, one emulated SM so that every launch
+"""Dry-run of bench.py's GPU arm on the CPU interpreter of the kernels (tiny sizes, one emulated SM so that every launch
 runs in this process and may write to ordinary host memory).  torch's CUDA entry points are stubbed: "device" tensors are
 host tensors.  Purpose: execute every line of the bench orchestration (legs, JSON assembly) before it meets a real GPU;
 the numbers it prints mean nothing.   usage: python tests/emu/run_bench_on_emu.py [bench args]"""

@@ -1,7 +1,7 @@
 """Runs pytest on the GPU parity suite with the ctypes binding pointed at tests/emu/libmeshnav_emu.so.
 
 Test infrastructure: the CUDA kernels' sources, compiled unchanged by g++ against the CPU interpreter in this directory,
-are driven through the same C ABI and compared with the oracle exactly as `-m gpu` does on a B200 (small meshes only).
+are driven through the same C ABI and compared with the oracle exactly as `-m gpu` does on an H100 (small meshes only).
 Usage: python tests/emu/run_suite.py <pytest args>"""
 import os
 import subprocess

@@ -1,5 +1,5 @@
 """CPU tests of the drop-in boundary: the C-ABI library loads, exports every symbol the header
-declares, and FAILS LOUDLY (no fallback) when no sm_100 device is present."""
+declares, and FAILS LOUDLY (no fallback) when no sm_90 device is present."""
 import ctypes as C
 import os
 import re
@@ -27,7 +27,7 @@ def test_header_symbols_exported():
 
 
 def test_no_cpu_fallback_without_gpu():
-    """Without a usable sm_100 device mnb_create must fail (MNB_E_CUDA) -- nothing routes to a CPU path."""
+    """Without a usable sm_90 device mnb_create must fail (MNB_E_CUDA) -- nothing routes to a CPU path."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present: the loud-failure path is exercised on the CPU-only build box")
@@ -62,4 +62,4 @@ def test_product_never_loads_the_cpu_interpreter():
                 assert "libmeshnav_emu" not in src and "tests.emu" not in src and "tests/emu" not in src, f
     blob = open(os.path.join(pkg, "libmeshnav_b200.so"), "rb").read()
     assert b"mnb_emu_switch" not in blob and b"mnb-emu" not in blob
-    assert b"sm_100" in blob, "the shipped library carries no sm_100a code"
+    assert b"sm_90a" in blob, "the shipped library carries no sm_90a code"

@@ -4,7 +4,7 @@ launches) and the whole `-m gpu` parity suite is replayed on it through the C AB
 
 What this does and does not prove: control flow, indexing, the band engine's round logic, sub-warp shuffles, stage /
 sweep bookkeeping and every host-side entry point are exercised bit-for-bit against the oracle; timing, occupancy and
-memory-ordering (fences) are not modelled -- `-m gpu` on a B200 remains the parity gate.  The interpreter is test
+memory-ordering (fences) are not modelled -- `-m gpu` on an H100 remains the parity gate.  The interpreter is test
 infrastructure: it is never loaded by the mesh_navigation_b200 package (tests/test_abi.py checks that)."""
 import os
 import subprocess
@@ -90,7 +90,7 @@ def test_cpp_host_mirror_on_the_cpu_interpreter(emu_lib, tmp_path, oracle_mod):
 
 
 def test_bench_orchestration_on_the_cpu_interpreter(emu_lib):
-    """bench.py's B200 arm, every leg, executed end to end on the interpreter at toy sizes (tests/emu/run_bench_on_emu.py):
+    """bench.py's GPU arm, every leg, executed end to end on the interpreter at toy sizes (tests/emu/run_bench_on_emu.py):
     the JSON line must carry the contract's keys and no secondary leg may have fallen into its error branch"""
     import json
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "emu", "run_bench_on_emu.py"), "--size", "90", "--batch-size", "50",
@@ -110,14 +110,14 @@ def test_bench_orchestration_on_the_cpu_interpreter(emu_lib):
     assert line["other_kernels"]["dynamic_obstacle_update"]["incremental_equals_full"] is True
     v = line["other_kernels"]["optin_variants"]
     assert v["layers_prefetching_walk_vs_round1_walk"]["identical"] and v["inflation_clean_candidate_skip"]["identical"]
-    # the parity blocks of the driver-run line: timed plan, config-3 plan, sampled batch fields
+    # the parity blocks of the bench line: timed plan, config-3 plan, sampled batch fields
     assert line["config"]["parity"]["ok"] and line["config"]["parity"]["n_mismatch"] == 0
     assert line["config"]["config3"]["parity"]["ok"] and line["config"]["batched"]["parity_sampled"]["ok"]
     assert "parity_failed" not in line
 
 
 def test_smoke_entry_on_the_cpu_interpreter(emu_lib):
-    """__graft_entry__.smoke() (the driver's GPU smoke check) with the binding pointed at the interpreted kernels"""
+    """__graft_entry__.smoke() (the GPU smoke check) with the binding pointed at the interpreted kernels"""
     code = ("import sys; sys.path.insert(0, %r); from mesh_navigation_b200 import _lib; _lib.LIB_PATH = %r; "
             "import __graft_entry__ as g; g.smoke()") % (ROOT, emu_lib)
     r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, capture_output=True, text=True, timeout=600,

@@ -1,7 +1,6 @@
 """Multi-GPU entry points of the C ABI (mnb_group_*, mnb_cvp_batch_sharded; include/meshnav_b200.h): one process, N devices,
 goal k on rank k mod N, fields all-gathered by NCCL inside the library.  Runs with every device count the box offers (a
-single device exercises the sharding / layout code without NCCL; the N = 2 run on the 2-GPU box is recorded in
-profiles/r02_group_n2.md)."""
+single device exercises the sharding / layout code without NCCL)."""
 import ctypes as C
 
 import numpy as np

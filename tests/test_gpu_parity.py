@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): every call goes through the C ABI
+"""GPU parity tests (run with -m gpu on an H100): every call goes through the C ABI
 (libmeshnav_b200.so) and is compared with the CPU oracle on the same seeded inputs.
 
 Bars (north_star): Dijkstra distances bit-identical and predecessors bit-exact;

@@ -1,7 +1,7 @@
 """Dev script (no GPU): bit-parity of the whole-grid CVP kernel vs the oracle on a LARGE mesh, run on the CPU interpreter
 of the kernels (tests/emu).  `python tools/emu_big_parity.py 3200` = 10.24 M vertices: ~2 min map build, ~3 min wavefront
 with MNB_EMU_SMS=8, ~25 GB of RAM.  This is the case that exposed the exact-key-tie ordering defect (4 potentials off by
-1 ulp, on the B200 and on the interpreter alike) and that verifies its fix (0 mismatches)."""
+1 ulp, on the GPU and on the interpreter alike) and that verifies its fix (0 mismatches)."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -1,7 +1,7 @@
 """Dev script (GPU box): A/B of the opt-in variants written without GPU access (round 1), one call, ~2 GPU-minutes.
   python tools/gpu_ab.py [grid side of the single-plan mesh, default 2240]
 Prints, for each variant, kernel time + the bit-equality against the default kernel:
-  * clean-candidate skip: whole-grid single CVP plan (5 M) and the per-CTA batch (1 M, 296 goals = one wave)
+  * clean-candidate skip: whole-grid single CVP plan (5 M) and the per-CTA batch (1 M, 2 goals per SM = one wave)
   * k_layers<true> (shared-memory seen-set) on the 5 M mesh
   * the dynamic-obstacle cycle (inflation update, vector field, incremental layerChanged vs full re-install)"""
 import ctypes as C, sys, time
@@ -71,10 +71,11 @@ nb = 1000
 bpos, bfaces = synth.grid_mesh(nb, nb, terrain=True)
 bm = MeshMap(bpos, bfaces); bm.setCosts(np.zeros(bm.V, np.float32), bm.edgeDistances())
 bm.L.mnb_debug_set_skip_clean.argtypes = [C.c_void_p, C.c_int32]
-goals = synth.batch_goal_vertices(bm.V, 296, seed=1234)
+G = 2 * torch.cuda.get_device_properties(0).multi_processor_count     # one wave: 2 CTAs per SM
+goals = synth.batch_goal_vertices(bm.V, G, seed=1234)
 gi, gj = np.minimum(goals % nb, nb - 2), np.minimum(goals // nb, nb - 2)
 sfs = (2 * (gj * (nb - 1) + gi)).astype(np.uint32); sps = bpos[bfaces[sfs]].mean(1).astype(np.float32)
-out = torch.empty((296, bm.V), dtype=torch.float32, device='cuda')
+out = torch.empty((G, bm.V), dtype=torch.float32, device='cuda')
 bref = None
 for skip in (0, 1, 0, 1):
     bm.L.mnb_debug_set_skip_clean(bm._ctx, skip)
@@ -85,8 +86,8 @@ for skip in (0, 1, 0, 1):
     st = bm.stats()
     cur = out[:8].cpu().numpy()
     if bref is None: bref = cur.copy()
-    print(f"[batch 296 x 1M] skip_clean={skip}: {1e3*dt:.1f} ms -> {296/dt:.1f} plans/s, kernel {st['kernel_ms']:.1f} ms, recomputes/V {st['recomputes']/296/bm.V:.2f} "
-          f"skipped/V {st['skipped']/296/bm.V:.2f} first 8 fields != default: {int((cur.view(np.uint32) != bref.view(np.uint32)).sum())}", flush=True)
+    print(f"[batch {G} x 1M] skip_clean={skip}: {1e3*dt:.1f} ms -> {G/dt:.1f} plans/s, kernel {st['kernel_ms']:.1f} ms, recomputes/V {st['recomputes']/G/bm.V:.2f} "
+          f"skipped/V {st['skipped']/G/bm.V:.2f} first 8 fields != default: {int((cur.view(np.uint32) != bref.view(np.uint32)).sum())}", flush=True)
 bm.L.mnb_debug_set_skip_clean(bm._ctx, 0)
 for delta in (0.2, 0.3, 0.45, 0.6):
     bm.set_tuning(delta, 1, 0)
@@ -95,5 +96,5 @@ for delta in (0.2, 0.3, 0.45, 0.6):
         t = time.perf_counter(); bm.cvp_batch_dev(sfs, sps, 1.0, out.data_ptr()); torch.cuda.synchronize(); dt = time.perf_counter() - t
     bm.use_device_pointers(False)
     st = bm.stats()
-    print(f"[batch 296 x 1M] delta={delta}: {1e3*dt:.1f} ms -> {296/dt:.1f} plans/s, recomputes/V {st['recomputes']/296/bm.V:.2f} rounds/plan {st['rounds']/296:.0f}", flush=True)
+    print(f"[batch {G} x 1M] delta={delta}: {1e3*dt:.1f} ms -> {G/dt:.1f} plans/s, recomputes/V {st['recomputes']/G/bm.V:.2f} rounds/plan {st['rounds']/G:.0f}", flush=True)
 bm.close()

@@ -1,11 +1,11 @@
-"""Dev script (GPU box): band-width sweep of the single-plan kernels on a large terrain (config 5: 7072 -> 50 M vertices).
+"""Dev script (GPU box): band-width sweep of the single-plan kernels on a large terrain (config 5: 5000 -> 25 M vertices).
   python tools/gpu_c5_sweep.py [grid side] [comma list of band widths in mean edge weights]"""
 import sys, zlib
 import numpy as np
 sys.path.insert(0, '.')
 from mesh_navigation_b200 import synth
 from mesh_navigation_b200.api import MeshMap, CVPMeshPlanner, DijkstraMeshPlanner
-n = int(sys.argv[1]) if len(sys.argv) > 1 else 7072
+n = int(sys.argv[1]) if len(sys.argv) > 1 else 5000
 ks = [float(x) for x in (sys.argv[2] if len(sys.argv) > 2 else "0,6,10,14,28").split(",")]
 pos, faces = synth.grid_mesh(n, n, terrain=True)
 mm = MeshMap(pos, faces)

@@ -1,11 +1,11 @@
 """Dev script (GPU box, under ncu): one launch each of the fused layers, the single-plan CVP wavefront and the single-plan
-Dijkstra wavefront on the config-5 terrain (7072 x 7072 = 50 M vertices)."""
+Dijkstra wavefront on the config-5 terrain (5000 x 5000 = 25 M vertices)."""
 import sys
 import numpy as np
 sys.path.insert(0, '.')
 from mesh_navigation_b200 import synth
 from mesh_navigation_b200.api import MeshMap, CVPMeshPlanner, DijkstraMeshPlanner
-n = int(sys.argv[1]) if len(sys.argv) > 1 else 7072
+n = int(sys.argv[1]) if len(sys.argv) > 1 else 5000
 pos, faces = synth.grid_mesh(n, n, terrain=True)
 mm = MeshMap(pos, faces)
 ed = mm.edgeDistances(); mm.setCosts(np.zeros(mm.V, np.float32), ed)
