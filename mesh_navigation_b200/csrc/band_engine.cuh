@@ -58,6 +58,8 @@ constexpr int STAGNATION_ROUNDS = 24;
 // float32 potentials collide millions of times on 10M-vertex meshes, hence the ids at every level: without them a
 // cascade under a tied key was ordered after ALL plain labels of that key.
 constexpr uint32_t EXT_POOL = 0x80000000u;
+constexpr uint32_t ELL_W = 8;          // slots of an ELL row (problems.cuh: one face / edge per slot)
+constexpr int ELL_EMPTY = -1;          // an unused slot
 struct EvTime { float a1, a2, a3; uint32_t root, ext, self; };
 __device__ __forceinline__ EvTime ev_normal(float key, uint32_t id) { EvTime t; t.a1 = key; t.a2 = 0.0f; t.a3 = 0.0f; t.root = id; t.ext = 0u; t.self = id; return t; }
 // per-vertex label: one 16-byte word {d, a1, a2 | root flag, a3 | ext flag}
@@ -345,17 +347,25 @@ struct SweepStage {
 };
 constexpr uint32_t SEEN_NEVER = 0xffffffffu;
 
-__device__ __forceinline__ unsigned int stage_push(Stage& st, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
-  const unsigned int p = atomicAdd(&st.n, 1u);
+__device__ __forceinline__ void stage_put(Stage& st, unsigned int p, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
   if (p < Stage::CAP) st.buf[p] = v;
   else list_next[atomicAdd(count_next, 1u)] = v;  // overflow: straight to global
+}
+__device__ __forceinline__ unsigned int stage_push(Stage& st, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
+  const unsigned int p = atomicAdd(&st.n, 1u);
+  stage_put(st, p, v, list_next, count_next);
   return p;
 }
-// same, and registers the slot for the in-round sweeps with the version its vertex had at the last evaluation
+// same into slot p (reserved by the caller), and registers the slot for the in-round sweeps with the version its vertex had
+// at the last evaluation
+__device__ __forceinline__ void stage_put_seen(Stage& st, SweepStage& ss, unsigned int p, uint32_t v, uint32_t seen, const uint4& label_bits,
+                                               uint32_t* list_next, unsigned int* count_next) {
+  stage_put(st, p, v, list_next, count_next);
+  if (p < Stage::SW_CAP) { ss.seen[p] = seen; ss.lab[p] = label_bits; }
+}
 __device__ __forceinline__ void stage_push_seen(Stage& st, SweepStage& ss, uint32_t v, uint32_t seen, const uint4& label_bits,
                                                 uint32_t* list_next, unsigned int* count_next) {
-  const unsigned int p = stage_push(st, v, list_next, count_next);
-  if (p < Stage::SW_CAP) { ss.seen[p] = seen; ss.lab[p] = label_bits; }
+  stage_put_seen(st, ss, atomicAdd(&st.n, 1u), v, seen, label_bits, list_next, count_next);
 }
 
 // flush the CTA stage to the global list (all threads of the CTA call this)
@@ -580,6 +590,14 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
                                      const float band_end_init, const uint32_t max_rounds, const int n_sweeps_arg,
                                      SweepStage* ss, const uint32_t n_vertices) {
   const int n_sweeps = SW ? n_sweeps_arg : 0;
+  // CVP on the whole grid: the main pass hands each candidate to ONE thread first (P::eval_plain, ~400 candidates per CTA
+  // and round on the 5M terrain -- seven serial batches of the 64 a CTA holds on 8 lanes each) and queues the few it
+  // cannot take for the 8-lane evaluation.  The sweeps keep the 8-lane form: ~65 dirty candidates per CTA and sweep are
+  // one batch, and a thread walking its faces one by one takes longer than 8 lanes taking one face each.
+  constexpr bool FAST = SW && P::PLAIN_FAST;
+  __shared__ uint32_t gq[FAST ? Stage::SW_CAP : 1];
+  __shared__ unsigned int gq_n;
+  if constexpr (FAST) { if (threadIdx.x == 0) gq_n = 0; __syncthreads(); }
   bool rescanned = false;
   float band_end_prev = band_end_init;
   unsigned long long my_recomputes = 0, my_settled = 0, my_skipped = 0;
@@ -737,12 +755,32 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     // ... and dealt round-robin (candidate i -> CTA i mod nblk): the list is ordered by flush time, i.e. by how busy the
     // producing CTA was, so contiguous chunks would hand all the "hot" candidates (the ones whose labels are still
     // moving) to a few CTAs while the rest idle at the barrier
+    // converged prefix: the sequential algorithm has popped c with exactly this label
+    auto settle = [&](const uint32_t c, const Label& old) {
+      mark[c] = MARK_FIXED;
+      my_settled++;
+      if (has_robot && (c == r0 || c == r1 || c == r2)) {
+        if (atomicSub(&ctl->robot_left, 1) == 1) {
+          float bd = old.d; EvTime bt = old.t;
+          const uint32_t rv[3] = {r0, r1, r2};
+          for (int k = 0; k < 3; ++k) {
+            const Label so = prob.load_label(rv[k]);
+            if (prob.tless(bt, so.t)) { bt = so.t; bd = so.d; }
+          }
+          ctl->goal_time[0] = __float_as_uint(bt.a1); ctl->goal_time[1] = bt.root; ctl->goal_time[2] = __float_as_uint(bt.a2);
+          ctl->goal_time[3] = __float_as_uint(bt.a3); ctl->goal_time[4] = bt.ext; ctl->goal_time[5] = bt.self;
+          atomicMin(&ctl->goal_ring[(r + 1) & 1], __float_as_uint((float)((double)bd + goal_dist_offset)));
+        }
+      }
+    };
     const unsigned int cnt = n > blk ? (n - blk + nblk - 1) / nblk : 0u;
-    for (unsigned int qb = (threadIdx.x >> 5) * 4u; qb < cnt; qb += (blockDim.x >> 3)) {
+    // the 8-lane main pass over cnt_g candidates: the CTA's share of the round's list or (queued) the entries of gq
+    auto main_pass8 = [&](const unsigned int cnt_g, const bool queued) {
+    for (unsigned int qb = (threadIdx.x >> 5) * 4u; qb < cnt_g; qb += (blockDim.x >> 3)) {
       const unsigned int q = qb + ((threadIdx.x & 31) >> 3);
-      bool has = q < cnt;
+      bool has = q < cnt_g;
       uint32_t c = 0;
-      if (has) c = __ldcg(&list_r[(size_t)q * nblk + blk]);
+      if (has) c = queued ? gq[q] : __ldcg(&list_r[(size_t)q * nblk + blk]);
       // issue the independent loads of the candidate together: its label, its ELL row, its mark (and version)
       Label old = prob.load_label(has ? c : 0u);
       int4 ix = prob.load_row_idx(has ? c : 0u, j);
@@ -750,25 +788,9 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       const uint32_t mk = __ldcg(&mark[has ? c : 0u]);
       uint32_t v0 = 0;
       if constexpr (SW) if (n_sweeps > 0) v0 = __ldcg(&prob.ver[has ? c : 0u]);
-      const float d = old.d, tau = old.t.a1;
+      const float tau = old.t.a1;
       if (has && tau < m_prev && tau < band_end_prev && tau < settle_cap) {
-        if (j == 0) {
-          mark[c] = MARK_FIXED;
-          my_settled++;
-          if (has_robot && (c == r0 || c == r1 || c == r2)) {
-            if (atomicSub(&ctl->robot_left, 1) == 1) {
-              float bd = d; EvTime bt = old.t;
-              const uint32_t rv[3] = {r0, r1, r2};
-              for (int k = 0; k < 3; ++k) {
-                const Label so = prob.load_label(rv[k]);
-                if (prob.tless(bt, so.t)) { bt = so.t; bd = so.d; }
-              }
-              ctl->goal_time[0] = __float_as_uint(bt.a1); ctl->goal_time[1] = bt.root; ctl->goal_time[2] = __float_as_uint(bt.a2);
-            ctl->goal_time[3] = __float_as_uint(bt.a3); ctl->goal_time[4] = bt.ext; ctl->goal_time[5] = bt.self;
-            atomicMin(&ctl->goal_ring[(r + 1) & 1], __float_as_uint((float)((double)bd + goal_dist_offset)));
-            }
-          }
-        }
+        if (j == 0) settle(c, old);
         has = false;
       }
       if constexpr (P::CAN_SKIP) if (skip_ok && has) {
@@ -786,6 +808,115 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
         }
       }
       evaluate(has, c, old, ix, w, mk, v0, true, 0u);
+    }
+    };
+    if constexpr (FAST) {
+      // One thread per candidate (P::eval_plain) with the side effects of evaluate(); what it cannot take goes to gq for the
+      // 8-lane evaluation.  Strict rounds (back-steps are deferred) and rounds with an armed goal cutoff (sources beyond it
+      // do not expand) evaluate everything on 8 lanes.  The stage pushes are warp-aggregated: with every thread of the CTA
+      // pushing at the same moment, per-thread atomics on the one shared counter serialise.
+      constexpr unsigned FULL = 0xffffffffu;
+      const uint32_t lane = threadIdx.x & 31u, lt = (1u << lane) - 1u;
+      const bool fast_round = !prob.strict && !(has_robot && goal_b != INF_BITS);
+      for (unsigned int cb = 0; cb < cnt; cb += (unsigned)Stage::SW_CAP) {
+        const unsigned int ce = min(cnt, cb + (unsigned)Stage::SW_CAP);
+        for (unsigned int ib = cb + (threadIdx.x & ~31u); ib < ce; ib += blockDim.x) {      // warp-uniform trip count
+          const unsigned int i = ib + lane;
+          bool has = i < ce;
+          uint32_t c = 0u, mk = MARK_FIXED, v0 = 0u;
+          uint4 ob = make_uint4(0u, 0u, 0u, 0u);
+          if (has) {
+            c = __ldcg(&list_r[(size_t)i * nblk + blk]);
+            ob = __ldcg(&prob.state[c]);
+            mk = __ldcg(&mark[c]);
+            if (n_sweeps > 0) v0 = __ldcg(&prob.ver[c]);
+            const float tau = __uint_as_float(ob.y);
+            if (tau < m_prev && tau < band_end_prev && tau < settle_cap) { settle(c, prob.unpack_label(c, ob)); has = false; }
+          }
+          float m = 0.0f, excl;
+          const bool done = has && fast_round &&
+              P::eval_plain(prob.ell_idx, prob.ell_w, prob.ell_geo, prob.invalid, prob.state, prob.seed_max_d, band_end, c, m, excl);
+          const uint32_t mb = __float_as_uint(m);
+          const uint4 nb = make_uint4(mb, mb, 0u, 0u);                  // c pops at (m, c)
+          uint32_t won = 0u;                                             // ring slots (2k + source) this thread activated
+          if (done) {
+            const bool changed = ob.x != mb || ob.y != mb || ob.z != 0u || ob.w != 0u;
+            my_recomputes++;
+            if (changed) {
+              if (ob.x != INF_BITS) __stcg(&prob.chg[c], r + 1u);
+              __stcg(&prob.state[c], nb);
+              my_mtau = fminf(my_mtau, fminf(__uint_as_float(ob.y), m));
+            }
+            my_lo = fminf(my_lo, m);
+            const bool act = mb != INF_BITS && mk == MARK_CAND;
+            const bool bump = changed && n_sweeps > 0;
+            if (bump || act) {
+              // face neighbours: version bumps of a re-label, activation (once) of the unmarked ones -- the marks of the
+              // whole ring are requested first so that their loads overlap, only the unmarked neighbours take the CAS
+              uint32_t todo = 0u;
+              if (act) {
+#pragma unroll
+                for (int k = 0; k < (int)ELL_W; ++k) {
+                  const int4 ix = prob.load_row_idx(c, (uint32_t)k);
+                  if (ix.x == ELL_EMPTY) continue;
+                  if (__ldcg(&mark[(uint32_t)ix.x]) == MARK_NONE) todo |= 1u << (2 * k);
+                  if (__ldcg(&mark[(uint32_t)ix.y]) == MARK_NONE) todo |= 2u << (2 * k);
+                }
+              }
+#pragma unroll
+              for (int k = 0; k < (int)ELL_W; ++k) {
+                const int4 ix = prob.load_row_idx(c, (uint32_t)k);
+                if (ix.x == ELL_EMPTY) continue;
+                const uint32_t xs[2] = {(uint32_t)ix.x, (uint32_t)ix.y};
+#pragma unroll
+                for (int t = 0; t < 2; ++t) {
+                  const uint32_t x = xs[t];
+                  if (bump) atomicAdd(&prob.ver[x], 1u);
+                  if (((todo >> (2 * k + t)) & 1u) && prob.eligible(x) && atomicCAS(&mark[x], MARK_NONE, MARK_CAND) == MARK_NONE)
+                    won |= 1u << (2 * k + t);
+                }
+              }
+              if (act) mark[c] = MARK_CAND_ACT;
+            }
+          }
+          // stage slots of the warp: each thread's candidate and the neighbours it activated, one shared atomic
+          const unsigned int mine = (done ? 1u : 0u) + (unsigned)__popc(won);
+          unsigned int incl = mine;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(FULL, incl, o); if (lane >= (unsigned)o) incl += y; }
+          const unsigned int tot = __shfl_sync(FULL, incl, 31);
+          if (tot) {
+            unsigned int base = 0u;
+            if (lane == 0) base = atomicAdd(&st.n, tot);
+            unsigned int p = __shfl_sync(FULL, base, 0) + incl - mine;
+            if (done) stage_put_seen(st, *ss, p++, c, v0, nb, list_n, &ctl->count[next]);
+            for (; won; won &= won - 1u) {
+              const int b = __ffs(won) - 1;
+              const int4 ix = prob.load_row_idx(c, (uint32_t)(b >> 1));
+              stage_put_seen(st, *ss, p++, (b & 1) ? (uint32_t)ix.y : (uint32_t)ix.x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]);
+            }
+          }
+          const bool defer = has && !done;
+          const unsigned dq = __ballot_sync(FULL, defer);
+          if (dq) {
+            unsigned int qbase = 0u;
+            if (lane == 0) qbase = atomicAdd(&gq_n, (unsigned)__popc(dq));
+            qbase = __shfl_sync(FULL, qbase, 0);
+            if (defer) gq[qbase + __popc(dq & lt)] = c;
+          }
+        }
+        __syncthreads();
+        const unsigned int nq = gq_n;
+#ifdef MNB_GRID_TIMING
+        if (gtid == 0) { ctl->t_ph[1] += nq; ctl->t_ph[7] += (unsigned long long)(clock64() - tp0); }
+#endif
+        main_pass8(nq, true);
+        __syncthreads();
+        if (threadIdx.x == 0) gq_n = 0;
+        __syncthreads();
+      }
+    } else {
+      main_pass8(cnt, false);
     }
     // ---- in-round sweeps: the CTA keeps relaxing the candidates it staged (survivors + newly activated) whose
     // inputs changed since their last evaluation, so a dependency chain advances several hops per barrier ----

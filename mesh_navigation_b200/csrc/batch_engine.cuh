@@ -344,8 +344,8 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
       __syncthreads();
       const unsigned int nwork = wk.n;
       // ---------------- phase B: one THREAD per candidate, plain causal evaluations only ----------------
-      // The throughput form of the evaluation: a thread walks the faces of its candidate (ELL row), every source label plain,
-      // no possible seed, and the causal collapse applies (CvpEllProblemT::replay_sub8): d = min over the causal faces.
+      // The throughput form of the evaluation (CvpEllProblemT::eval_plain): a thread walks the faces of its candidate (ELL
+      // row), every source label plain, no possible seed, and the causal collapse applies: d = min over the causal faces.
       // ~25 warp-instructions per candidate instead of ~140 for the 8-lane form, 32 candidates per warp in flight.  Anything
       // else is deferred to phase C.
       for (unsigned int ib = (threadIdx.x & ~31u); ib < nwork; ib += blockDim.x) {
@@ -353,44 +353,11 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
         const bool has = i < nwork;
         bool defer = false;
         uint32_t ce = 0u, c = 0u; uint4 ob = make_uint4(0u, 0u, 0u, 0u);
-        float m = INF, tmin_nc = INF, excl = INF; int deg = 0;
+        float m = INF, excl = INF;
         if (has) {
           ce = wk.q[i]; c = ce & ~LIST_ACTIVATED;
           ob = __ldcg(&G.state[c]);
-          if (strict) defer = true;
-          for (int k = 0; k < (int)ELL_W && !defer; ++k) {
-            const int4 ix = __ldg(&a.ell_idx[(size_t)c * ELL_W + k]);
-            if (k == 0) { deg = ix.w; if (deg > (int)ELL_W) { defer = true; break; } }
-            if (ix.x == ELL_EMPTY) continue;
-            const uint32_t v1 = (uint32_t)ix.x, v2 = (uint32_t)ix.y;
-            const uint4 sa = __ldcg(&G.state[v1]), sb = __ldcg(&G.state[v2]);
-            const float da = __uint_as_float(sa.x), db = __uint_as_float(sb.x);
-            if (((sa.z | sa.w | sb.z | sb.w) >> 31) || da <= sd.seed_max || db <= sd.seed_max) { defer = true; break; }
-            if (a.invalid && (a.invalid[v1] || a.invalid[v2])) continue;
-            if (sa.x != INF_BITS && !(da < band_end)) excl = fminf(excl, da);
-            if (sb.x != INF_BITS && !(db < band_end)) excl = fminf(excl, db);
-            if (!(da < band_end) || !(db < band_end)) continue;
-            const float ta = __uint_as_float(sa.y), tb = __uint_as_float(sb.y);
-            const bool v1_later = tb < ta || (tb == ta && v2 < v1);
-            const float T1 = v1_later ? ta : tb;
-            const float4 w = __ldg(&a.ell_w[(size_t)c * ELL_W + k]);
-            // the static part of the unfolding (apex of the triangle, cosine at v3) is recomputed from the three weights instead of
-            // being read from the precomputed table: 256 of the 512 bytes a vertex' ELL rows occupy, and the rows -- not the
-            // labels -- are what makes the hot set of a few hundred concurrent wavefronts overflow the L2 (MNB_BATCH_GEO_TABLE=1
-            // at compile time restores the table read)
-            double U, X;
-#ifdef MNB_BATCH_GEO_TABLE
-            const double2* gp = reinterpret_cast<const double2*>(a.ell_geo) + 2 * ((size_t)c * ELL_W + k);
-            const double2 g01 = __ldg(gp), g23 = __ldg(gp + 1);
-            CvpEllProblemT<false>::FaceGeo fg; fg.p = g01.x; fg.hc = g01.y; fg.t0a = g23.x;
-            CvpEllProblemT<false>::eval_face_geo((double)da, (double)db, (double)w.z, (double)w.y, (double)w.x, fg, U, X);
-#else
-            CvpEllProblemT<false>::eval_face((double)da, (double)db, (double)w.z, (double)w.y, (double)w.x, U, X);
-#endif
-            const float Xf = (float)X;
-            if (Xf > T1 && U <= X) m = fminf(m, Xf); else tmin_nc = fminf(tmin_nc, T1);
-          }
-          if (!defer && __float_as_uint(tmin_nc) != INF_BITS && !(tmin_nc > m)) defer = true;   // a non-causal face that may fire first
+          defer = strict || !CvpEllProblemT<false>::eval_plain(a.ell_idx, a.ell_w, a.ell_geo, a.invalid, G.state, sd.seed_max, band_end, c, m, excl);
         }
         const bool done = has && !defer;
         bool changed = false, act_now = false;

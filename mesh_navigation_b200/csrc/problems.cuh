@@ -208,8 +208,6 @@ struct CvpProblem : LabelStore {
 // unfolding) concurrently; the reference's event order is then replayed across the
 // lanes with shuffles.  Vertices with more than 8 faces take the CSR path on lane 0.
 // ---------------------------------------------------------------------------
-constexpr uint32_t ELL_W = 8;
-constexpr int ELL_EMPTY = -1;
 
 template <bool SKIP>
 struct CvpEllProblemT : CvpProblem {
@@ -218,6 +216,8 @@ struct CvpEllProblemT : CvpProblem {
   // through `d < band_end`); it is re-evaluated only if a source was re-labelled in or after the round of its last
   // evaluation.  Both stamps are 1-based round numbers and only ever compared across a group barrier.
   static constexpr bool CAN_SKIP = SKIP;      // compile-time: the default instantiation carries none of the bookkeeping
+  // whole-grid main pass: plain causal candidates one per thread (eval_plain), the rest on 8 lanes (run_band_rounds_sub8)
+  static constexpr bool PLAIN_FAST = !SKIP;
   uint32_t* last_eval;     // round + 1 of the last evaluation; 0 = never evaluated
   uint32_t* dirty_round;   // round + 1 of the last re-label of a face neighbour; 0 = never
   uint32_t* excl_min;      // float bits: smallest finite source label that lay beyond the band end at the last evaluation and
@@ -255,6 +255,54 @@ struct CvpEllProblemT : CvpProblem {
     else if (fabs(t0a) <= 1 && acos_less(t1a, t0a) && acos_less(t2a, t0a)) { X = u3tmp; return; }   // |t0a| > 1: acos(t0a) is NaN in the reference
     else fb = acos_less(t1a, t2a) ? 1 : 2;
     X = (fb == 1) ? (u1 + b) : (u2 + a);
+  }
+
+  // The throughput form of replay_sub8's fast path: ONE thread walks the ELL row of c.  Every source label plain, no source
+  // that may be a seed, and the causal collapse applies: m = min over the causal faces, c pops at (m, c).  Returns false
+  // (c needs the general evaluation) for more than 8 faces, a cascade member among the sources, a possible seed, or a
+  // non-causal face that may fire before c pops.  excl: smallest finite source label beyond the band end.
+  // Strict rounds and an armed goal cutoff are the caller's to exclude.
+  __device__ __forceinline__ static bool eval_plain(const int4* __restrict__ ell_idx, const float4* __restrict__ ell_w,
+                                                    const double4* __restrict__ ell_geo, const uint8_t* __restrict__ invalid,
+                                                    const uint4* state, float seed_max, float band_end, uint32_t c,
+                                                    float& m, float& excl) {
+    (void)ell_geo;
+    const float INF = __uint_as_float(INF_BITS);
+    float tmin_nc = INF;
+    m = INF; excl = INF;
+    for (int k = 0; k < (int)ELL_W; ++k) {
+      const int4 ix = __ldg(&ell_idx[(size_t)c * ELL_W + k]);
+      if (k == 0 && ix.w > (int)ELL_W) return false;
+      if (ix.x == ELL_EMPTY) continue;
+      const uint32_t v1 = (uint32_t)ix.x, v2 = (uint32_t)ix.y;
+      const uint4 sa = __ldcg(&state[v1]), sb = __ldcg(&state[v2]);
+      const float da = __uint_as_float(sa.x), db = __uint_as_float(sb.x);
+      if (((sa.z | sa.w | sb.z | sb.w) >> 31) || da <= seed_max || db <= seed_max) return false;
+      if (invalid && (invalid[v1] || invalid[v2])) continue;
+      if (sa.x != INF_BITS && !(da < band_end)) excl = fminf(excl, da);
+      if (sb.x != INF_BITS && !(db < band_end)) excl = fminf(excl, db);
+      if (!(da < band_end) || !(db < band_end)) continue;
+      const float ta = __uint_as_float(sa.y), tb = __uint_as_float(sb.y);
+      const bool v1_later = tb < ta || (tb == ta && v2 < v1);
+      const float T1 = v1_later ? ta : tb;
+      const float4 w = __ldg(&ell_w[(size_t)c * ELL_W + k]);
+      // the static part of the unfolding (apex of the triangle, cosine at v3) is recomputed from the three weights instead of
+      // being read from the precomputed table: 256 of the 512 bytes a vertex' ELL rows occupy, and the rows -- not the
+      // labels -- are what makes the hot set of a few hundred concurrent wavefronts overflow the L2 (MNB_BATCH_GEO_TABLE=1
+      // at compile time restores the table read)
+      double U, X;
+#ifdef MNB_BATCH_GEO_TABLE
+      const double2* gp = reinterpret_cast<const double2*>(ell_geo) + 2 * ((size_t)c * ELL_W + k);
+      const double2 g01 = __ldg(gp), g23 = __ldg(gp + 1);
+      FaceGeo fg; fg.p = g01.x; fg.hc = g01.y; fg.t0a = g23.x;
+      eval_face_geo((double)da, (double)db, (double)w.z, (double)w.y, (double)w.x, fg, U, X);
+#else
+      eval_face((double)da, (double)db, (double)w.z, (double)w.y, (double)w.x, U, X);
+#endif
+      const float Xf = (float)X;
+      if (Xf > T1 && U <= X) m = fminf(m, Xf); else tmin_nc = fminf(tmin_nc, T1);
+    }
+    return __float_as_uint(tmin_nc) == INF_BITS || tmin_nc > m;     // no non-causal face may fire first
   }
 
   template <class F>
@@ -753,6 +801,7 @@ struct DijkstraProblem : TimeAlg {
 struct DijkstraEllProblem : DijkstraProblem {
   static constexpr bool TWO_SOURCES = false;
   static constexpr bool CAN_SKIP = false;     // one relaxation is as cheap as the bookkeeping of skipping it
+  static constexpr bool PLAIN_FAST = false;
   uint32_t* last_eval = nullptr; uint32_t* dirty_round = nullptr; uint32_t* excl_min = nullptr; int skip_clean = 0;
   static constexpr bool prefetch_marks = true;
   const uint4* __restrict__ ell_adj;
