@@ -97,6 +97,19 @@ int32_t mnb_set_costs(mnb_ctx* ctx, const float* vertex_costs /* V */, const flo
 int32_t mnb_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_vertex, double cost_limit,
                      double goal_dist_offset, float* out_dist, uint32_t* out_pred);
 
+/* Batched full-field Dijkstra: n independent DijkstraMeshPlanner::dijkstra waves (dijkstra_mesh_planner.cpp:217-398,
+ * robot vertex -1) on the installed map, hundreds of them in flight at once.  Row k of out_dist / out_pred ([n][V]
+ * row-major) is the field seeded at seed_vertices[k], bit-identical to mnb_dijkstra(ctx, seed_vertices[k], -1,
+ * cost_limit, ...): +inf / self where unreached.  Either output may be NULL, not both; duplicate seeds are allowed.
+ * A predecessor row is the whole shortest-path tree towards its seed: walking pred from any vertex gives its path.
+ * seed_vertices is always a host pointer; the outputs follow mnb_set_pointer_mode.  MNB_INVALID_START if a seed is
+ * >= V (checked before anything is written).  The number of concurrent waves is capped by the free device memory
+ * (16 bytes per vertex and wave), so a large map runs with fewer of them.  The waves use a workspace of their own: the
+ * results of the last mnb_cvp (mnb_cvp_backtrack, mnb_vector_map with pred = NULL) and of the last inflation
+ * (mnb_inflation_vector_map) remain available after this call. */
+int32_t mnb_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices /* n, host */, double cost_limit,
+                           float* out_dist /* [n][V] or NULL */, uint32_t* out_pred /* [n][V] or NULL */);
+
 /* ---- CVPMeshPlanner::waveFrontPropagation (cvp_mesh_planner.cpp:651-886) -
  * seed_face / seed_pos = the reference's start_face / start (navigation goal, :673,:719-728)
  * robot_face           = the reference's goal_face (:674) or -1 for a full field.

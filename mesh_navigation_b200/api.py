@@ -220,6 +220,12 @@ class MeshMap:
         return self._check(self.L.mnb_dijkstra(self._ctx, int(seed_vertex), int(robot_vertex), float(cost_limit),
                                                float(goal_dist_offset), _p(d_dist), _p(d_pred)))
 
+    def dijkstra_batch_dev(self, seed_vertices, cost_limit, d_dist: int, d_pred: int = 0) -> int:
+        """mnb_dijkstra_batch with device outputs ([n,V] rows; 0 = not wanted); the seeds are host values"""
+        sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32)
+        return self._check(self.L.mnb_dijkstra_batch(self._ctx, sv.size, _p(sv), float(cost_limit),
+                                                     _p(d_dist) if d_dist else None, _p(d_pred) if d_pred else None))
+
     def cvp_dev(self, seed_face, seed_pos, robot_face, cost_limit, goal_dist_offset, d_dist: int, d_pred: int = 0,
                 d_dir: int = 0, d_cut: int = 0) -> int:
         sp = np.ascontiguousarray(seed_pos, dtype=np.float32)
@@ -248,6 +254,16 @@ class DijkstraMeshPlanner:
         pred = np.empty(m.V, dtype=np.uint32)
         rc = m._check(m.L.mnb_dijkstra(m._ctx, int(seed_vertex), int(robot_vertex), float(self.cost_limit),
                                        float(self.goal_dist_offset), _p(dist), _p(pred)))
+        return dict(outcome=rc, dist=dist, pred=pred, **m.stats())
+
+    def dijkstraBatch(self, seed_vertices, want_pred: bool = True):
+        """full-field dijkstra() (robot vertex -1) for every seed in one call: row k of dist / pred ([n,V]) equals
+        dijkstra(seed_vertices[k])'s; pred is None unless want_pred"""
+        m = self.map
+        sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32).reshape(-1)
+        dist = np.empty((sv.size, m.V), dtype=np.float32)
+        pred = np.empty((sv.size, m.V), dtype=np.uint32) if want_pred else None
+        rc = m._check(m.L.mnb_dijkstra_batch(m._ctx, sv.size, _p(sv), float(self.cost_limit), _p(dist), _p(pred)))
         return dict(outcome=rc, dist=dist, pred=pred, **m.stats())
 
     def computeVectorMap(self, pred):

@@ -436,6 +436,87 @@ __global__ void __launch_bounds__(512, 1) k_dijkstra(const DijkstraKernelArgs a)
   for (uint32_t v = gtid; v < V; v += gthreads) a.out_dist[v] = __uint_as_float(state[v].x);
 }
 
+// Batches of full-field Dijkstra plans (mnb_dijkstra_batch): the outer loop of k_cvp_batch around the round loop of
+// k_dijkstra.  One wavefront per CTA (CS = 1) or per cluster of CS CTAs; persistent groups pull seed indices from an
+// atomic counter and stop taking new ones once the cancel flag is set.  A wavefront owns only what the round loop reads:
+// the float label (tau = d), the marks, two candidate lists and its GroupCtl -- 16 bytes per vertex.  Row q of the
+// outputs is written by the group that ran seed q; out_pred (may be null) doubles as the problem's predecessor array.
+struct DijkstraBatchWorkspace {   // per group (index g): label + g*V etc.
+  float* label;
+  uint32_t* mark;
+  uint32_t* list0;
+  uint32_t* list1;
+  GroupCtl* ctl;
+};
+constexpr size_t DIJKSTRA_BATCH_BYTES_PER_VERTEX = sizeof(float) + 3 * sizeof(uint32_t);
+
+struct DijkstraBatchArgs {
+  uint32_t V;
+  const uint32_t* adj_ptr; const uint2* adj_nw;
+  const float* cost; const uint8_t* invalid;
+  DijkstraBatchWorkspace ws;
+  uint32_t n_queries;
+  const uint32_t* seeds;        // [n_queries] device
+  double cost_limit;
+  float delta;
+  float* out_dist;              // [n_queries][V] or null
+  uint32_t* out_pred;           // [n_queries][V] or null
+  unsigned int* next_query;
+  const int* cancel_flag;
+  uint32_t max_rounds;
+};
+
+template <int CS>
+__global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijkstra_batch(const DijkstraBatchArgs a) {
+  __shared__ Stage st;
+  uint32_t g, gthreads, gtid;
+  group_coords<CS>(g, gthreads, gtid);
+  const uint32_t V = a.V;
+  float* label = a.ws.label + (size_t)g * V;
+  uint32_t* mark = a.ws.mark + (size_t)g * V;
+  uint32_t* list0 = a.ws.list0 + (size_t)g * V;
+  uint32_t* list1 = a.ws.list1 + (size_t)g * V;
+  GroupCtl* ctl = a.ws.ctl + g;
+  const volatile int* cancel = a.cancel_flag;
+  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  __syncthreads();
+  DijkstraProblemT<float> prob;
+  prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
+  prob.state = label; prob.cost_limit = a.cost_limit; prob.deferred_m = __uint_as_float(INF_BITS);
+  for (;;) {
+    if (gtid == 0) ctl->query = (cancel && *cancel) ? a.n_queries : atomicAdd(a.next_query, 1u);
+    group_sync<CS>();
+    const uint32_t q = __ldcg(&ctl->query);
+    if (q >= a.n_queries) break;
+    uint32_t* pred = a.out_pred ? a.out_pred + (size_t)q * V : nullptr;
+    for (uint32_t v = gtid; v < V; v += gthreads) {
+      label[v] = __uint_as_float(INF_BITS); mark[v] = MARK_NONE;
+      if (pred) pred[v] = v;                                   // dijkstra:268-269
+    }
+    group_sync<CS>();
+    prob.pred = pred;
+    const uint32_t s = a.seeds[q];
+    if (gtid == 0) {
+      label[s] = 0.0f;                                         // dijkstra:276
+      mark[s] = MARK_FIXED;
+      unsigned int n0 = 0;
+      prob.activate(s, [&](uint32_t x) {
+        if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
+      });
+      ctl_reset(ctl, n0, 0.0f);
+    }
+    group_sync<CS>();
+    run_band_rounds<CS>(prob, ctl, list0, list1, mark, st, a.delta, gthreads, gtid, 0, 0xffffffffu, 0xffffffffu, 0xffffffffu,
+                        0.0, a.cancel_flag, 1e-30f, a.max_rounds);
+    group_sync<CS>();
+    if (a.out_dist) {
+      float* od = a.out_dist + (size_t)q * V;
+      for (uint32_t v = gtid; v < V; v += gthreads) od[v] = __ldcg(&label[v]);
+    }
+    group_sync<CS>();
+  }
+}
+
 // Single Dijkstra plan on the whole GPU: 8 lanes per candidate (one edge each), wide band + in-round sweeps,
 // same engine instance as k_cvp_grid.
 __global__ void __launch_bounds__(512, 1) k_dijkstra_grid(const DijkstraKernelArgs a) {

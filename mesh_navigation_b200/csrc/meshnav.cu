@@ -26,6 +26,10 @@ using namespace mnb;
 #include "kernels_updates.cuh"
 #include "kernels_raycast.cuh"
 
+// default band width of the batched Dijkstra planner in mean edge weights: on the 1 M terrain with 1024 goals 1.5 w was
+// fastest of 1 - 10 w (DESIGN §5)
+constexpr float DIJKSTRA_BATCH_DELTA_W = 1.5f;
+
 // ============================================================================
 // host side
 // ============================================================================
@@ -50,6 +54,9 @@ struct mnb_ctx {
   // workspace
   uint32_t ws_groups = 0;
   WaveWorkspace ws{};
+  uint32_t dws_groups = 0;       // the batched Dijkstra planner's own workspace (k_dijkstra_batch)
+  DijkstraBatchWorkspace dws{};
+  uint32_t* d_batch_pred = nullptr; size_t batch_pred_cap = 0;    // its predecessor rows in host-pointer mode
   unsigned int* d_next_query = nullptr;
   int* h_cancel = nullptr; int* d_cancel = nullptr;
   // scratch outputs for host-pointer mode
@@ -88,9 +95,11 @@ struct mnb_ctx {
   int sweeps = -1;             // in-round sweeps of the whole-grid single-plan kernel; -1 = derived from the band width
   float grid_delta = 1.8f;     // band width of the whole-grid single-plan kernel (wide band + in-round sweeps)
   float dijkstra_grid_delta = 3.0f;
+  float dijkstra_batch_delta = 0.18f;
   // The band widths above are potentials, i.e. multiples of the edge weights: unless the caller fixed them (mnb_set_tuning
   // with band_delta > 0) they follow the mean finite edge weight w of the installed weights -- 2.5 w for batches, 20 w for a
-  // single CVP plan, 25 w for a single Dijkstra plan, less on maps above ~12 M vertices (install_weights); one dependency hop is
+  // single CVP plan, 25 w for a single Dijkstra plan, less on maps above ~12 M vertices, DIJKSTRA_BATCH_DELTA_W w for
+  // Dijkstra batches (install_weights); one dependency hop is
   // ~1.35 w (the in-round sweeps are counted in hops).  On the 0.1 m bench meshes (w = 0.118) that is 0.3 / 2.4 / 3.0 m, the values
   // the kernels were tuned with.
   bool delta_explicit = false; float w_mean = 0.0f; double* d_wsum = nullptr;
@@ -127,6 +136,8 @@ static void free_mesh(mnb_ctx* c) {
   dfree(c->d_edge_dist); dfree(c->d_edge_w); dfree(c->d_cost); dfree(c->d_invalid); dfree(c->d_wsum);
   dfree(c->ws.state); dfree(c->ws.ext); dfree(c->ws.pool); dfree(c->ws.skipw); dfree(c->ws.root); dfree(c->ws.last_eval); dfree(c->ws.dirty); dfree(c->ws.excl); dfree(c->ws.chg); dfree(c->ws.ver); dfree(c->ws.mark); dfree(c->ws.list0); dfree(c->ws.list1); dfree(c->ws.ctl);
   c->ws_groups = 0;
+  dfree(c->dws.label); dfree(c->dws.mark); dfree(c->dws.list0); dfree(c->dws.list1); dfree(c->dws.ctl); c->dws_groups = 0;
+  dfree(c->d_batch_pred); c->batch_pred_cap = 0;
   dfree(c->d_out_dist); c->out_dist_cap = 0; dfree(c->d_out_pred); dfree(c->d_out_dir); dfree(c->d_out_cut);
   dfree(c->d_infl_invalid); dfree(c->d_out_cost);
   dfree(c->d_infl_vec); dfree(c->d_infl_dist); dfree(c->d_infl_src); dfree(c->d_infl_flag);
@@ -228,7 +239,10 @@ uint32_t mnb_num_edges(mnb_ctx* ctx) { return ctx ? ctx->E : 0; }
 
 int32_t mnb_set_tuning(mnb_ctx* ctx, float band_delta, int32_t cluster_size, int32_t threads_per_cta) {
   if (!ctx) return MNB_E_ARG;
-  if (band_delta > 0) { ctx->delta = band_delta; ctx->grid_delta = band_delta; ctx->dijkstra_grid_delta = band_delta; ctx->delta_explicit = true; }
+  if (band_delta > 0) {
+    ctx->delta = band_delta; ctx->grid_delta = band_delta; ctx->dijkstra_grid_delta = band_delta; ctx->dijkstra_batch_delta = band_delta;
+    ctx->delta_explicit = true;
+  }
   if (cluster_size == 1 || cluster_size == 2 || cluster_size == 4 || cluster_size == 8 || cluster_size == 16) {
     ctx->cluster = cluster_size;
     ctx->batch_cluster = cluster_size > 8 ? 8 : cluster_size;
@@ -364,6 +378,7 @@ static int32_t install_weights(mnb_ctx* ctx) {
     ctx->delta = 2.5f * ctx->w_mean;
     ctx->grid_delta = fminf(20.0f, k) * ctx->w_mean;
     ctx->dijkstra_grid_delta = fminf(25.0f, k) * ctx->w_mean;
+    ctx->dijkstra_batch_delta = DIJKSTRA_BATCH_DELTA_W * ctx->w_mean;
   }
   ctx->costs_set = true;
   return MNB_OK;
@@ -524,6 +539,20 @@ static cudaError_t launch_cooperative(void (*kern)(const KArgs), const KArgs& ar
 #endif
 }
 
+// free and total device memory (sizes the workspaces that are capped by memory)
+static cudaError_t device_memory(int device, size_t* free_b, size_t* total_b) {
+#ifdef MNB_EMU_ACTIVE
+  // the CPU interpreter of the kernels (tests/emu) models no memory budget: its whole arena counts as free
+  cudaDeviceProp prop;
+  const cudaError_t e = cudaGetDeviceProperties(&prop, device);
+  *free_b = prop.totalGlobalMem; *total_b = prop.totalGlobalMem;
+  return e;
+#else
+  (void)device;
+  return cudaMemGetInfo(free_b, total_b);
+#endif
+}
+
 static int32_t launch_cvp(mnb_ctx* ctx, const CvpKernelArgs& a, int cs, unsigned groups) {
   cudaError_t e;
   const unsigned blocks = groups * cs;
@@ -539,9 +568,9 @@ static int32_t launch_cvp(mnb_ctx* ctx, const CvpKernelArgs& a, int cs, unsigned
   return MNB_OK;
 }
 
-static int32_t finish_stats(mnb_ctx* ctx, unsigned groups, unsigned launches) {
+static int32_t finish_stats(mnb_ctx* ctx, unsigned groups, unsigned launches, const GroupCtl* ctl = nullptr) {
   std::vector<GroupCtl> h(groups);
-  CK(cudaMemcpyAsync(h.data(), ctx->ws.ctl, sizeof(GroupCtl) * groups, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.data(), ctl ? ctl : ctx->ws.ctl, sizeof(GroupCtl) * groups, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->stats.rounds = 0; ctx->stats.recomputes = 0; ctx->stats.settled = 0;
   ctx->stats.skipped = 0; ctx->stats.deep_labels = 0; ctx->stats.pool_words = 0;
@@ -781,6 +810,82 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   if ((rc = finish_stats(ctx, 1, 1)) != MNB_OK) return rc;
   if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
   if (robot_vertex >= 0 && rp == (uint32_t)robot_vertex) return MNB_NO_PATH_FOUND;          // dijkstra:358-362
+  return MNB_SUCCESS;
+}
+
+// n full-field Dijkstra waves in one launch (k_dijkstra_batch).  The waves run in a workspace of their own, so the
+// results of the last mnb_cvp (predecessors, directions, cutting faces) and the labels of the last inflation stay valid.
+static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, float* out_dist,
+                                   uint32_t* out_pred) {
+  if (!ctx || !seed_vertices || (!out_dist && !out_pred) || !ctx->V || n == 0) return MNB_E_ARG;
+  if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
+  for (uint32_t i = 0; i < n; ++i) if (seed_vertices[i] >= ctx->V) return MNB_INVALID_START;
+  CK(cudaSetDevice(ctx->device));
+  int32_t rc;
+  const size_t V = ctx->V;
+  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
+  if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized)
+    if (out_dist && (rc = ensure_out(ctx, (size_t)n * V, false)) != MNB_OK) return rc;
+    if (out_pred && (size_t)n * V > ctx->batch_pred_cap) {
+      dfree(ctx->d_batch_pred); ctx->batch_pred_cap = 0;
+      CK(dalloc(&ctx->d_batch_pred, (size_t)n * V)); ctx->batch_pred_cap = (size_t)n * V;
+    }
+  }
+  // concurrent wavefronts: the CTA slots of the kernel, capped by the device memory their workspace may take
+  int per_sm = 1;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_dijkstra_batch<1>, MNB_BATCH_THREADS, 0));
+  if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
+  if (per_sm < 1) per_sm = 1;
+  const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
+  size_t free_b = 0, total_b = 0;
+  CK(device_memory(ctx->device, &free_b, &total_b));
+  const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
+  const size_t avail = free_b + (size_t)ctx->dws_groups * per_group;    // a larger workspace replaces the current one
+  const size_t reserve = std::max<size_t>((size_t)512 << 20, total_b / 32);
+  const size_t mem_groups = avail > reserve ? (avail - reserve) / per_group : 0;
+  if (mem_groups == 0) { ctx->err = "not enough free device memory for one Dijkstra wavefront"; return MNB_E_NOMEM; }
+  const unsigned want = (unsigned)std::min<size_t>(std::min<size_t>(n, slots), mem_groups);
+  // CTAs per wavefront: one when the wavefronts fill the machine, a cluster when there are fewer of them than CTA slots
+  int cs = ctx->batch_cluster;
+  if (cs <= 0) { cs = 1; while (cs < 8 && (unsigned)(2 * cs) * want <= slots) cs *= 2; }
+  unsigned groups = std::min(want, std::max(1u, slots / (unsigned)cs));
+  if (groups > ctx->dws_groups) {
+    dfree(ctx->dws.label); dfree(ctx->dws.mark); dfree(ctx->dws.list0); dfree(ctx->dws.list1); dfree(ctx->dws.ctl); ctx->dws_groups = 0;
+    const size_t m = (size_t)groups * V;
+    CK(dalloc(&ctx->dws.label, m)); CK(dalloc(&ctx->dws.mark, m)); CK(dalloc(&ctx->dws.list0, m)); CK(dalloc(&ctx->dws.list1, m));
+    CK(dalloc(&ctx->dws.ctl, groups));
+    ctx->dws_groups = groups;
+  }
+  if (ctx->h_cancel) *ctx->h_cancel = 0;     // dijkstra:238
+  if ((rc = ensure_adj_tables(ctx)) != MNB_OK) return rc;
+  CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_vertices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
+  CK(cudaMemsetAsync(ctx->dws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+  DijkstraBatchArgs a{};
+  a.V = ctx->V; a.adj_ptr = ctx->d_adj_ptr; a.adj_nw = ctx->d_adj_nw; a.cost = ctx->d_cost;
+  a.invalid = ctx->has_invalid ? ctx->d_invalid : nullptr; a.ws = ctx->dws;
+  a.n_queries = n; a.seeds = ctx->d_seed_faces; a.cost_limit = cost_limit; a.delta = ctx->dijkstra_batch_delta;
+  a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
+  a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
+  a.next_query = ctx->d_next_query; a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V);
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  cudaError_t e;
+  const unsigned blocks = groups * (unsigned)cs;
+  switch (cs) {
+    case 1: e = launch_cluster(k_dijkstra_batch<1>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+    case 2: e = launch_cluster(k_dijkstra_batch<2>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+    case 4: e = launch_cluster(k_dijkstra_batch<4>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+    default: e = launch_cluster(k_dijkstra_batch<8>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+  }
+  if (e != cudaSuccess) { ctx->err = std::string("dijkstra batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  if (!dev) {
+    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if ((rc = finish_stats(ctx, groups, 1, ctx->dws.ctl)) != MNB_OK) return rc;
+  if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
   return MNB_SUCCESS;
 }
 
@@ -1231,6 +1336,10 @@ int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, cons
 int32_t mnb_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_vertex, double cost_limit, double goal_dist_offset,
                      float* out_dist, uint32_t* out_pred) {
   return guarded(ctx, [&]() { return impl_dijkstra(ctx, seed_vertex, robot_vertex, cost_limit, goal_dist_offset, out_dist, out_pred); });
+}
+int32_t mnb_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, float* out_dist,
+                           uint32_t* out_pred) {
+  return guarded(ctx, [&]() { return impl_dijkstra_batch(ctx, n, seed_vertices, cost_limit, out_dist, out_pred); });
 }
 int32_t mnb_inflate(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid,
                     const mnb_inflation_params* params, float* out_dist, float* out_cost) {

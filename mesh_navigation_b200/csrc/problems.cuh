@@ -1,5 +1,6 @@
 // Per-algorithm "pull" recompute rules plugged into the band engine.
 #pragma once
+#include <type_traits>
 #include "band_engine.cuh"
 
 namespace mnb {
@@ -734,8 +735,12 @@ struct InflationProblem : LabelStore {
 // dijkstra_mesh_planner.cpp:332): order (d[u], u).  Edge weights are >= 0 so a
 // vertex always pops at its own key: tau = d, one level.
 //   adj_nw[k] = {neighbour id, float bits of the edge weight}
+// The label word S is the engine's uint4 {d, tau, -, -} or, in the lean workspace of the batch kernel
+// (k_dijkstra_batch), the float d alone: tau = d carries no information of its own.
+// pred may be null: no predecessors are written.
 // ---------------------------------------------------------------------------
-struct DijkstraProblem : TimeAlg {
+template <class S>
+struct DijkstraProblemT : TimeAlg {
   static constexpr bool HAS_GOAL_TIME = false;    // edge weights >= 0: vertices pop in potential order, the test on the value is exact
   static constexpr bool CAN_SKIP = false;
   static constexpr int STAGNATION = STAGNATION_ROUNDS;
@@ -743,15 +748,23 @@ struct DijkstraProblem : TimeAlg {
   const uint2* __restrict__ adj_nw;
   const float* __restrict__ cost;
   const uint8_t* __restrict__ invalid;  // may be null
-  uint4* state;
+  S* state;
   uint32_t* pred;
   double cost_limit;
   float deferred_m;                     // unused (edge weights >= 0: no back-steps), kept for the engine interface
   int strict;
 
+  __device__ __forceinline__ static float label_d(const uint4& s) { return __uint_as_float(s.x); }
+  __device__ __forceinline__ static float label_d(float s) { return s; }
+  __device__ __forceinline__ static float label_tau(const uint4& s) { return __uint_as_float(s.y); }
+  __device__ __forceinline__ static float label_tau(float s) { return s; }
+  __device__ __forceinline__ void store_d(uint32_t c, float d) const {
+    if constexpr (std::is_same<S, float>::value) __stcg(&state[c], d);
+    else __stcg(&state[c], make_uint4(__float_as_uint(d), __float_as_uint(d), 0u, 0u));
+  }
   __device__ __forceinline__ Label load_label(uint32_t v) const {
-    const uint4 s = __ldcg(&state[v]);
-    Label l; l.d = __uint_as_float(s.x); l.t = ev_normal(__uint_as_float(s.y), v);
+    const S s = __ldcg(&state[v]);
+    Label l; l.d = label_d(s); l.t = ev_normal(label_tau(s), v);
     return l;
   }
   __device__ __forceinline__ bool eligible(uint32_t x) const { return !(invalid && invalid[x]); }  // :328
@@ -769,7 +782,7 @@ struct DijkstraProblem : TimeAlg {
     for (uint32_t k = kb; k < ke; ++k) {
       const uint2 nw = __ldg(&adj_nw[k]);
       const uint32_t u = nw.x;
-      const float du = __uint_as_float(__ldcg(&state[u]).x);
+      const float du = label_d(__ldcg(&state[u]));
       if (!(du < band_end)) continue;
       if (du > goal) continue;                               // :299
       if ((double)__ldg(&cost[u]) > cost_limit) continue;    // :302
@@ -782,14 +795,15 @@ struct DijkstraProblem : TimeAlg {
     nd = best; ntau = best;
     if (__float_as_uint(nd) == __float_as_uint(old.d)) {
       // same potential; the predecessor can still change among exact ties
-      if (__float_as_uint(nd) != INF_BITS && pred[c] != best_u) pred[c] = best_u;
+      if (pred && __float_as_uint(nd) != INF_BITS && pred[c] != best_u) pred[c] = best_u;
       return false;
     }
-    __stcg(&state[c], make_uint4(__float_as_uint(nd), __float_as_uint(ntau), 0u, 0u));
-    pred[c] = best_u;
+    store_d(c, nd);
+    if (pred) pred[c] = best_u;
     return true;
   }
 };
+using DijkstraProblem = DijkstraProblemT<uint4>;
 
 
 // ---------------------------------------------------------------------------
