@@ -123,6 +123,25 @@ int32_t mnb_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64
 int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n, host */,
                       const float* seed_pos /* 3n, host */, double cost_limit, float* out_dist);
 
+/* Batched full-field CVP vector fields: n independent goals, like mnb_cvp_batch, with the inputs of the vector field as
+ * well.  Row k of each output ([n][V] row-major) is bit-identical to the same output of mnb_cvp(ctx, seed_faces[k],
+ * &seed_pos[3k], -1, cost_limit, ...): potential (+inf = unreached), predecessor (self = none), direction (0 = none)
+ * and cutting face (-1 = none; a seed vertex has itself, 0 and the seed face).  Any output may be NULL, not all of them;
+ * duplicate goals are allowed.  Rows k of pred / direction / cutting face feed mnb_vector_map(ctx, pred_k, dir_k,
+ * cut_k, out), which is CVPMeshPlanner::computeVectorMap (cvp_mesh_planner.cpp:204-239): one vector field per goal,
+ * e.g. one per robot of a fleet.  seed_faces / seed_pos are always host pointers; the outputs follow
+ * mnb_set_pointer_mode.  MNB_INVALID_START if a seed face is >= F (checked before anything is written); MNB_CANCELED
+ * after mnb_cancel (the rows are then incomplete).  With out_dist alone the call runs mnb_cvp_batch's kernel; with any
+ * other output each wave derives its rows before it takes the next goal.  The number of concurrent waves is capped by the free
+ * device memory (~76 bytes per vertex and wave) as well as by the CTA slots, so a large map runs with fewer of them;
+ * MNB_E_NOMEM if not even one fits.  The waves share the wavefront workspace with mnb_cvp and the inflation wave: the
+ * last inflation's labels are dropped (as after mnb_cvp_batch), while the outputs of the last mnb_cvp
+ * (mnb_cvp_backtrack, mnb_vector_map with pred = NULL) remain available. */
+int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n, host */,
+                             const float* seed_pos /* 3n, host */, double cost_limit,
+                             float* out_dist /* [n][V] or NULL */, uint32_t* out_pred /* [n][V] or NULL */,
+                             float* out_direction /* [n][V] or NULL */, int32_t* out_cutting_face /* [n][V] or NULL */);
+
 /* ---- InflationLayer::waveCostInflation (inflation_layer.cpp:341-491) -----
  * lethals[n] (any order, duplicates allowed).  Uses edge_distances (:383), not edge_weights.
  * out_dist[V]: distances_ (+inf = not in the sparse map); out_cost[V]: riskiness_ =

@@ -239,6 +239,15 @@ class MeshMap:
         sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
         return self._check(self.L.mnb_cvp_batch(self._ctx, sf.size, _p(sf), _p(sp), float(cost_limit), _p(d_out)))
 
+    def cvp_batch_fields_dev(self, seed_faces, seed_pos, cost_limit, d_dist: int, d_pred: int = 0, d_dir: int = 0,
+                             d_cut: int = 0) -> int:
+        """mnb_cvp_batch_fields with device outputs ([n,V] rows; 0 = not wanted); the seeds are host values"""
+        sf = np.ascontiguousarray(seed_faces, dtype=np.uint32)
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
+        opt = lambda d: _p(d) if d else None
+        return self._check(self.L.mnb_cvp_batch_fields(self._ctx, sf.size, _p(sf), _p(sp), float(cost_limit), opt(d_dist),
+                                                       opt(d_pred), opt(d_dir), opt(d_cut)))
+
 
 class DijkstraMeshPlanner:
     """dijkstra_mesh_planner::DijkstraMeshPlanner -- wavefront part (dijkstra():217-398)."""
@@ -328,6 +337,22 @@ class CVPMeshPlanner:
         out = np.empty((sf.size, m.V), dtype=np.float32)
         rc = m._check(m.L.mnb_cvp_batch(m._ctx, sf.size, _p(sf), _p(sp), float(self.cost_limit), _p(out)))
         return dict(outcome=rc, dist=out, **m.stats())
+
+    def waveFrontPropagationBatchFields(self, seed_faces, seed_pos, want=("dist", "pred", "direction", "cutting_face")):
+        """full-field waveFrontPropagation (robot face -1) for every goal in one call: row k of each [n,V] array equals
+        waveFrontPropagation(seed_faces[k], seed_pos[k])'s; outputs not in `want` are None.  Rows k of pred, direction
+        and cutting_face give goal k's vector field through computeVectorMap."""
+        m = self.map
+        sf = np.ascontiguousarray(seed_faces, dtype=np.uint32).reshape(-1)
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
+        kinds = dict(dist=np.float32, pred=np.uint32, direction=np.float32, cutting_face=np.int32)
+        unknown = set(want) - set(kinds)
+        if unknown:
+            raise ValueError(f"unknown outputs {sorted(unknown)}; choose from {list(kinds)}")
+        out = {k: (np.empty((sf.size, m.V), dtype=t) if k in want else None) for k, t in kinds.items()}
+        rc = m._check(m.L.mnb_cvp_batch_fields(m._ctx, sf.size, _p(sf), _p(sp), float(self.cost_limit), _p(out["dist"]),
+                                               _p(out["pred"]), _p(out["direction"]), _p(out["cutting_face"])))
+        return dict(outcome=rc, **out, **m.stats())
 
 
 class InflationLayer:

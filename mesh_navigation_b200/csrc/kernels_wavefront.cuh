@@ -188,7 +188,62 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
 #ifndef MNB_BATCH_MINBLOCKS
 #define MNB_BATCH_MINBLOCKS 4
 #endif
-template <int CS>
+
+// The CVP epilogue: predecessors_ / direction_ / cutting_faces_ (cvp:423-431,493-517) from the FINAL labels of a wavefront.
+// Every vertex replays its faces once more in event order and evaluates the winning face with the literal acos form.  Done
+// after the wavefront so that the stored angles use the final source potentials.  Run by k_cvp_epilogue for a single plan
+// and by k_cvp_batch<CS, true> for each goal of a batch, on the wavefront's own workspace group.
+// The problem object: the workspace group's labels, the goal's seed face sf, the goal cutoff's pop time (not armed: +inf)
+// and the outputs (any may be null).
+__device__ __forceinline__ void cvp_epilogue_problem(const CvpKernelArgs& a, uint4* state, uint32_t* ext, uint32_t* root, uint32_t* chg,
+                                                     uint32_t* pool, GroupCtl* ctl, uint32_t sf, const EvTime& goal_t,
+                                                     uint32_t* pred, float* dir, int32_t* cut, CvpProblem& prob) {
+  prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
+  prob.state = state; prob.ext_arr = ext; prob.root_arr = root; prob.chg = chg;
+  prob.pool_w = pool; prob.pool = pool; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
+  prob.ver = nullptr; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = pred; prob.dir = dir; prob.cut = cut; prob.cost_limit = a.cost_limit;
+  prob.strict = 0;
+  prob.s0 = a.faces[3 * (size_t)sf]; prob.s1 = a.faces[3 * (size_t)sf + 1]; prob.s2 = a.faces[3 * (size_t)sf + 2];
+  prob.seed_noexpand = 0;
+  prob.goal_t = goal_t;
+  const uint32_t sv[3] = {prob.s0, prob.s1, prob.s2};
+  for (int k = 0; k < 3; ++k)
+    if (((double)a.cost[sv[k]] >= a.cost_limit) || (a.invalid && a.invalid[sv[k]])) prob.seed_noexpand |= (1u << k);
+}
+
+// one vertex c of the epilogue (goal: the goal cutoff's potential, +inf when not armed)
+__device__ __forceinline__ void cvp_epilogue_vertex(CvpProblem& prob, GroupCtl* ctl, uint32_t sf, float goal, uint32_t c) {
+  const uint4 lw = __ldcg(&prob.state[c]);
+  const float d = __uint_as_float(lw.x);
+  // statistic: labels whose pop time has more than 3 cascade levels (their tails live in the level pool; exact)
+  if (__float_as_uint(d) != INF_BITS && (lw.w >> 31) && (__ldcg(&prob.ext_arr[c]) & EXT_POOL)) atomicAdd(&ctl->deep_labels, 1u);
+  if (prob.seed_index(c) >= 0) {                         // cvp:719-728
+    if (prob.pred) prob.pred[c] = c;
+    if (prob.dir) prob.dir[c] = 0.0f;
+    if (prob.cut) prob.cut[c] = (int32_t)sf;
+    return;
+  }
+  int win = -1; float nd, wu1 = 0, wu2 = 0; EvFull nt;
+  if (__float_as_uint(d) != INF_BITS && prob.eligible(c))
+    prob.replay(c, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, nd, nt, win, wu1, wu2);
+  prob.write_aux(c, win, wu1, wu2);
+}
+
+// k_cvp_batch<CS, true>: the epilogue of goal q over the group's workspace, rows q of out_pred / out_dir / out_cut (each may
+// be null).  Out of line: its frame (the replay holds a vertex's faces) does not weigh on the registers of the round loop.
+__device__ __noinline__ void batch_fields_epilogue(const CvpKernelArgs& a, const BatchGroup& G, uint32_t q, uint32_t gthreads, uint32_t gtid) {
+  const uint32_t V = a.V;
+  const size_t row = (size_t)q * V;
+  const uint32_t sf = a.seed_faces[q];
+  CvpProblem prob;
+  cvp_epilogue_problem(a, G.state, G.ext_arr, G.root_arr, G.chg, G.pool, G.ctl, sf, ev_normal(__uint_as_float(INF_BITS), 0u),
+                       a.out_pred ? a.out_pred + row : nullptr, a.out_dir ? a.out_dir + row : nullptr, a.out_cut ? a.out_cut + row : nullptr, prob);
+  for (uint32_t v = gtid; v < V; v += gthreads) cvp_epilogue_vertex(prob, G.ctl, sf, __uint_as_float(INF_BITS), v);
+}
+
+// FIELDS = false: potentials only (mnb_cvp_batch, and the whole-grid experiment CS = 0).  FIELDS = true (mnb_cvp_batch_fields):
+// each group also runs the epilogue of its goal before it takes the next one, and takes none once the cancel flag is set.
+template <int CS, bool FIELDS>
 __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_batch(const CvpKernelArgs a) {
   __shared__ BatchStage st;
   __shared__ BatchWork wk;
@@ -205,7 +260,10 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
   if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; wk.n = 0; wk.ns = 0; }
   __syncthreads();
   for (;;) {
-    if (gtid == 0) ctl->query = atomicAdd(a.next_query, 1u);
+    if (gtid == 0) {
+      if constexpr (FIELDS) ctl->query = (a.cancel_flag && *(const volatile int*)a.cancel_flag) ? a.n_queries : atomicAdd(a.next_query, 1u);
+      else ctl->query = atomicAdd(a.next_query, 1u);
+    }
     group_sync<CS>();
     const uint32_t q = __ldcg(&ctl->query);
     if (q >= a.n_queries) break;
@@ -254,6 +312,7 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
       float* od = a.out_dist + (size_t)q * V;
       for (uint32_t v = gtid; v < V; v += gthreads) od[v] = __uint_as_float(__ldcg(&G.state[v]).x);
     }
+    if constexpr (FIELDS) batch_fields_epilogue(a, G, q, gthreads, gtid);
     group_sync<CS>();
   }
 }
@@ -342,39 +401,17 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
     for (uint32_t v = gtid; v < V; v += gthreads) a.out_dist[v] = __uint_as_float(state[v].x);
 }
 
-// predecessors_ / direction_ / cutting_faces_ (cvp:423-431,493-517) from the FINAL labels: every vertex
-// replays its faces once more in event order and evaluates the winning face with the literal acos form.
-// Done after the wavefront so that the stored angles use the final source potentials.
+// the epilogue of a single plan (cvp_epilogue_problem above), one thread per vertex; the goal cutoff is the plan's
 __global__ void __launch_bounds__(256) k_cvp_epilogue(const CvpKernelArgs a, GroupCtl* ctl) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= a.V) return;
   const uint32_t sf = a.seed_faces[0];
+  EvTime goal_t;
+  goal_t.a1 = __uint_as_float(ctl->goal_time[0]); goal_t.root = ctl->goal_time[1]; goal_t.a2 = __uint_as_float(ctl->goal_time[2]);
+  goal_t.a3 = __uint_as_float(ctl->goal_time[3]); goal_t.ext = ctl->goal_time[4]; goal_t.self = ctl->goal_time[5];
   CvpProblem prob;
-  prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
-  prob.state = a.ws.state; prob.ext_arr = a.ws.ext; prob.root_arr = a.ws.root; prob.chg = a.ws.chg;
-  prob.pool_w = a.ws.pool; prob.pool = prob.pool_w; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
-  prob.ver = nullptr; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = a.out_pred; prob.dir = a.out_dir; prob.cut = a.out_cut; prob.cost_limit = a.cost_limit;
-  prob.s0 = a.faces[3 * (size_t)sf]; prob.s1 = a.faces[3 * (size_t)sf + 1]; prob.s2 = a.faces[3 * (size_t)sf + 2];
-  prob.seed_noexpand = 0;
-  prob.goal_t.a1 = __uint_as_float(ctl->goal_time[0]); prob.goal_t.root = ctl->goal_time[1]; prob.goal_t.a2 = __uint_as_float(ctl->goal_time[2]);
-  prob.goal_t.a3 = __uint_as_float(ctl->goal_time[3]); prob.goal_t.ext = ctl->goal_time[4]; prob.goal_t.self = ctl->goal_time[5];
-  {
-    const uint32_t sv[3] = {prob.s0, prob.s1, prob.s2};
-    for (int k = 0; k < 3; ++k)
-      if (((double)a.cost[sv[k]] >= a.cost_limit) || (a.invalid && a.invalid[sv[k]])) prob.seed_noexpand |= (1u << k);
-  }
-  const uint4 lw = a.ws.state[c];
-  const float d = __uint_as_float(lw.x);
-  // statistic: labels whose pop time has more than 3 cascade levels (their tails live in the level pool; exact)
-  if (__float_as_uint(d) != INF_BITS && (lw.w >> 31) && (a.ws.ext[c] & EXT_POOL)) atomicAdd(&ctl->deep_labels, 1u);
-  if (prob.seed_index(c) >= 0) {                         // cvp:719-728
-    a.out_pred[c] = c; a.out_dir[c] = 0.0f; a.out_cut[c] = (int32_t)sf;
-    return;
-  }
-  int win = -1; float nd, wu1 = 0, wu2 = 0; EvFull nt;
-  if (__float_as_uint(d) != INF_BITS && prob.eligible(c))
-    prob.replay(c, __uint_as_float(INF_BITS), __uint_as_float(ctl->goal_bits), 0xfffffff0u /* final labels: nothing is deferred */, nd, nt, win, wu1, wu2);
-  prob.write_aux(c, win, wu1, wu2);
+  cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, goal_t, a.out_pred, a.out_dir, a.out_cut, prob);
+  cvp_epilogue_vertex(prob, ctl, sf, __uint_as_float(ctl->goal_bits), c);
 }
 
 // start == goal (dijkstra_mesh_planner.cpp:252-255): the maps as the reference leaves them after clearing (:241-249)

@@ -56,7 +56,9 @@ struct mnb_ctx {
   WaveWorkspace ws{};
   uint32_t dws_groups = 0;       // the batched Dijkstra planner's own workspace (k_dijkstra_batch)
   DijkstraBatchWorkspace dws{};
-  uint32_t* d_batch_pred = nullptr; size_t batch_pred_cap = 0;    // its predecessor rows in host-pointer mode
+  uint32_t* d_batch_pred = nullptr; size_t batch_pred_cap = 0;    // its predecessor rows in host-pointer mode (and mnb_cvp_batch_fields')
+  float* d_batch_dir = nullptr; size_t batch_dir_cap = 0;         // mnb_cvp_batch_fields' direction and cutting-face rows in host-pointer mode
+  int32_t* d_batch_cut = nullptr; size_t batch_cut_cap = 0;
   unsigned int* d_next_query = nullptr;
   int* h_cancel = nullptr; int* d_cancel = nullptr;
   // scratch outputs for host-pointer mode
@@ -137,7 +139,7 @@ static void free_mesh(mnb_ctx* c) {
   dfree(c->ws.state); dfree(c->ws.ext); dfree(c->ws.pool); dfree(c->ws.skipw); dfree(c->ws.root); dfree(c->ws.last_eval); dfree(c->ws.dirty); dfree(c->ws.excl); dfree(c->ws.chg); dfree(c->ws.ver); dfree(c->ws.mark); dfree(c->ws.list0); dfree(c->ws.list1); dfree(c->ws.ctl);
   c->ws_groups = 0;
   dfree(c->dws.label); dfree(c->dws.mark); dfree(c->dws.list0); dfree(c->dws.list1); dfree(c->dws.ctl); c->dws_groups = 0;
-  dfree(c->d_batch_pred); c->batch_pred_cap = 0;
+  dfree(c->d_batch_pred); c->batch_pred_cap = 0; dfree(c->d_batch_dir); c->batch_dir_cap = 0; dfree(c->d_batch_cut); c->batch_cut_cap = 0;
   dfree(c->d_out_dist); c->out_dist_cap = 0; dfree(c->d_out_pred); dfree(c->d_out_dir); dfree(c->d_out_cut);
   dfree(c->d_infl_invalid); dfree(c->d_out_cost);
   dfree(c->d_infl_vec); dfree(c->d_infl_dist); dfree(c->d_infl_src); dfree(c->d_infl_flag);
@@ -150,15 +152,22 @@ static void free_mesh(mnb_ctx* c) {
   c->costs_set = false;
 }
 
+// level pool (band_engine.cuh): pop times with more than 3 cascade levels keep their tails here; 2 words per vertex
+// hold the deepest flooded pockets randomised testing has produced with room to spare; exhaustion is reported
+static uint32_t ws_pool_cap(uint32_t V) { return (uint32_t)std::min<size_t>(std::max<size_t>(65536, 2 * (size_t)V), 0x7fffffffu); }
+// device bytes of one group of the wavefront workspace (ensure_workspace): two 16-byte and nine 4-byte words per vertex,
+// the level pool and the GroupCtl -- 76 bytes per vertex on large maps
+static size_t ws_bytes_per_group(uint32_t V) {
+  return (size_t)V * (2 * sizeof(uint4) + 9 * sizeof(uint32_t)) + (size_t)ws_pool_cap(V) * sizeof(uint32_t) + sizeof(GroupCtl);
+}
+
 static int32_t ensure_workspace(mnb_ctx* ctx, uint32_t groups) {
   if (groups <= ctx->ws_groups) return MNB_OK;
   dfree(ctx->ws.state); dfree(ctx->ws.ext); dfree(ctx->ws.pool); dfree(ctx->ws.skipw); dfree(ctx->ws.root); dfree(ctx->ws.last_eval); dfree(ctx->ws.dirty); dfree(ctx->ws.excl); dfree(ctx->ws.chg); dfree(ctx->ws.ver); dfree(ctx->ws.mark); dfree(ctx->ws.list0); dfree(ctx->ws.list1); dfree(ctx->ws.ctl);
   ctx->ws_groups = 0;
   const size_t n = (size_t)groups * ctx->V;
   CK(dalloc(&ctx->ws.state, n)); CK(dalloc(&ctx->ws.ext, n)); CK(dalloc(&ctx->ws.skipw, n)); CK(dalloc(&ctx->ws.root, n)); CK(dalloc(&ctx->ws.last_eval, n)); CK(dalloc(&ctx->ws.dirty, n)); CK(dalloc(&ctx->ws.excl, n)); CK(dalloc(&ctx->ws.chg, n)); CK(dalloc(&ctx->ws.ver, (size_t)ctx->V)); CK(dalloc(&ctx->ws.mark, n)); CK(dalloc(&ctx->ws.list0, n)); CK(dalloc(&ctx->ws.list1, n));
-  // level pool (band_engine.cuh): pop times with more than 3 cascade levels keep their tails here; 2 words per vertex
-  // hold the deepest flooded pockets randomised testing has produced with room to spare; exhaustion is reported
-  ctx->ws.pool_cap = (uint32_t)std::min<size_t>(std::max<size_t>(65536, 2 * (size_t)ctx->V), 0x7fffffffu);
+  ctx->ws.pool_cap = ws_pool_cap(ctx->V);
   CK(dalloc(&ctx->ws.pool, (size_t)groups * ctx->ws.pool_cap));
   CK(dalloc(&ctx->ws.ctl, groups));
   ctx->ws_groups = groups;
@@ -553,6 +562,17 @@ static cudaError_t device_memory(int device, size_t* free_b, size_t* total_b) {
 #endif
 }
 
+// concurrent wavefronts the device memory allows for a workspace of per_group bytes per wavefront: the free memory plus the
+// `current` groups a larger workspace would replace, less a reserve (512 MB or 1/32 of the device); 0 if not even one fits
+static int32_t memory_capped_groups(mnb_ctx* ctx, size_t per_group, uint32_t current, size_t* groups) {
+  size_t free_b = 0, total_b = 0;
+  CK(device_memory(ctx->device, &free_b, &total_b));
+  const size_t avail = free_b + (size_t)current * per_group;
+  const size_t reserve = std::max<size_t>((size_t)512 << 20, total_b / 32);
+  *groups = avail > reserve ? (avail - reserve) / per_group : 0;
+  return MNB_OK;
+}
+
 static int32_t launch_cvp(mnb_ctx* ctx, const CvpKernelArgs& a, int cs, unsigned groups) {
   cudaError_t e;
   const unsigned blocks = groups * cs;
@@ -652,11 +672,11 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
     }
     if (ctx->grid_engine == 1 && robot_face < 0) {
       int per_sm = 1;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp_batch<0>, MNB_BATCH_THREADS, 0));
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp_batch<0, false>, MNB_BATCH_THREADS, 0));
       if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
       if (per_sm < 1) { ctx->err = "k_cvp_batch<0> cannot be resident"; return MNB_E_CUDA; }
       a.delta = ctx->grid2_delta_w * (ctx->w_mean > 0.0f ? ctx->w_mean : 0.12f);
-      CK(launch_cooperative(k_cvp_batch<0>, a, (unsigned)(ctx->sm_count * per_sm), MNB_BATCH_THREADS, ctx->stream));
+      CK(launch_cooperative(k_cvp_batch<0, false>, a, (unsigned)(ctx->sm_count * per_sm), MNB_BATCH_THREADS, ctx->stream));
     } else
     CK(launch_cooperative(k_cvp_grid<false>, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
   } else {
@@ -704,7 +724,7 @@ static int32_t impl_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_fac
   static const bool legacy = getenv("MNB_BATCH_LEGACY") != nullptr;
   int per_sm = 1;
   if (legacy) { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp<1, false>, MNB_CVP_THREADS, 0)); if (per_sm > 2) per_sm = 2; }
-  else { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp_batch<1>, MNB_BATCH_THREADS, 0)); if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS; }
+  else { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp_batch<1, false>, MNB_BATCH_THREADS, 0)); if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS; }
   if (per_sm < 1) per_sm = 1;
   const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
   // CTAs per wavefront: one when the goals fill the machine; with fewer goals than CTA slots a cluster of CTAs shares a
@@ -737,15 +757,105 @@ static int32_t impl_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_fac
     cudaError_t e;
     const unsigned blocks = groups * (unsigned)cs;
     switch (cs) {
-      case 1: e = launch_cluster(k_cvp_batch<1>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 2: e = launch_cluster(k_cvp_batch<2>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 4: e = launch_cluster(k_cvp_batch<4>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      default: e = launch_cluster(k_cvp_batch<8>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 1: e = launch_cluster(k_cvp_batch<1, false>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 2: e = launch_cluster(k_cvp_batch<2, false>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 4: e = launch_cluster(k_cvp_batch<4, false>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      default: e = launch_cluster(k_cvp_batch<8, false>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
     }
     if (e != cudaSuccess) { ctx->err = std::string("cvp batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (!dev) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)n * ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
+  if ((rc = finish_stats(ctx, groups, 1)) != MNB_OK) return rc;
+  if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
+  return MNB_SUCCESS;
+}
+
+// n full-field CVP plans with their vector-field inputs in one launch (k_cvp_batch<CS, true>): each wavefront runs the
+// epilogue of its goal before its group takes the next one.  Only potentials requested: the potentials-only kernel.  The
+// waves share the wavefront workspace with single plans and inflation (not the single plan's outputs), and their number
+// is capped by the free device memory as well as by the CTA slots.
+static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
+                                     float* out_dist, uint32_t* out_pred, float* out_dir, int32_t* out_cut) {
+  if (!ctx || !seed_faces || !seed_pos || (!out_dist && !out_pred && !out_dir && !out_cut) || !ctx->V || n == 0) return MNB_E_ARG;
+  if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
+  for (uint32_t i = 0; i < n; ++i) if (seed_faces[i] >= ctx->F) return MNB_INVALID_START;
+  CK(cudaSetDevice(ctx->device));
+  int32_t rc;
+  const size_t V = ctx->V, rows = (size_t)n * V;
+  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  const bool fields = out_pred || out_dir || out_cut;
+  if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
+  if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized; the
+                       // single plan's outputs stay untouched for mnb_cvp_backtrack / mnb_vector_map)
+    if (out_dist && (rc = ensure_out(ctx, rows, false)) != MNB_OK) return rc;
+    if (out_pred && rows > ctx->batch_pred_cap) {
+      dfree(ctx->d_batch_pred); ctx->batch_pred_cap = 0;
+      CK(dalloc(&ctx->d_batch_pred, rows)); ctx->batch_pred_cap = rows;
+    }
+    if (out_dir && rows > ctx->batch_dir_cap) {
+      dfree(ctx->d_batch_dir); ctx->batch_dir_cap = 0;
+      CK(dalloc(&ctx->d_batch_dir, rows)); ctx->batch_dir_cap = rows;
+    }
+    if (out_cut && rows > ctx->batch_cut_cap) {
+      dfree(ctx->d_batch_cut); ctx->batch_cut_cap = 0;
+      CK(dalloc(&ctx->d_batch_cut, rows)); ctx->batch_cut_cap = rows;
+    }
+  }
+  // concurrent wavefronts: the CTA slots of the kernel, capped by the device memory their workspace may take
+  int per_sm = 1;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fields ? k_cvp_batch<1, true> : k_cvp_batch<1, false>, MNB_BATCH_THREADS, 0));
+  if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
+  if (per_sm < 1) per_sm = 1;
+  const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
+  size_t mem_groups = 0;
+  if ((rc = memory_capped_groups(ctx, ws_bytes_per_group(ctx->V), ctx->ws_groups, &mem_groups)) != MNB_OK) return rc;
+  if (mem_groups == 0) { ctx->err = "not enough free device memory for one CVP wavefront"; return MNB_E_NOMEM; }
+  const unsigned want = (unsigned)std::min<size_t>(std::min<size_t>(n, slots), mem_groups);
+  // CTAs per wavefront: one when the wavefronts fill the machine, a cluster when there are fewer of them than CTA slots
+  int cs = ctx->batch_cluster;
+  if (cs <= 0) { cs = 1; while (cs < 8 && (unsigned)(2 * cs) * want <= slots) cs *= 2; }
+  const unsigned groups = std::min(want, std::max(1u, slots / (unsigned)cs));
+  if ((rc = ensure_workspace(ctx, groups)) != MNB_OK) return rc;
+  if (ctx->h_cancel) *ctx->h_cancel = 0;
+  ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
+  CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_faces, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
+  CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+  CvpKernelArgs a{};
+  fill_cvp_args(ctx, a);
+  a.n_queries = n; a.robot_face = -1; a.cost_limit = cost_limit; a.goal_dist_offset = 0.0;
+  a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
+  a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
+  a.out_dir = !out_dir ? nullptr : (dev ? out_dir : ctx->d_batch_dir);
+  a.out_cut = !out_cut ? nullptr : (dev ? out_cut : ctx->d_batch_cut);
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  cudaError_t e;
+  const unsigned blocks = groups * (unsigned)cs;
+  if (fields) {
+    switch (cs) {
+      case 1: e = launch_cluster(k_cvp_batch<1, true>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 2: e = launch_cluster(k_cvp_batch<2, true>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 4: e = launch_cluster(k_cvp_batch<4, true>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      default: e = launch_cluster(k_cvp_batch<8, true>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+    }
+  } else {
+    switch (cs) {
+      case 1: e = launch_cluster(k_cvp_batch<1, false>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 2: e = launch_cluster(k_cvp_batch<2, false>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      case 4: e = launch_cluster(k_cvp_batch<4, false>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+      default: e = launch_cluster(k_cvp_batch<8, false>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
+    }
+  }
+  if (e != cudaSuccess) { ctx->err = std::string("cvp batch fields launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  if (!dev) {
+    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_dir) CK(cudaMemcpyAsync(out_dir, a.out_dir, sizeof(float) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_cut) CK(cudaMemcpyAsync(out_cut, a.out_cut, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+  }
   if ((rc = finish_stats(ctx, groups, 1)) != MNB_OK) return rc;
   if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
   return MNB_SUCCESS;
@@ -838,12 +948,8 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
   if (per_sm < 1) per_sm = 1;
   const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
-  size_t free_b = 0, total_b = 0;
-  CK(device_memory(ctx->device, &free_b, &total_b));
-  const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
-  const size_t avail = free_b + (size_t)ctx->dws_groups * per_group;    // a larger workspace replaces the current one
-  const size_t reserve = std::max<size_t>((size_t)512 << 20, total_b / 32);
-  const size_t mem_groups = avail > reserve ? (avail - reserve) / per_group : 0;
+  size_t mem_groups = 0;
+  if ((rc = memory_capped_groups(ctx, DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl), ctx->dws_groups, &mem_groups)) != MNB_OK) return rc;
   if (mem_groups == 0) { ctx->err = "not enough free device memory for one Dijkstra wavefront"; return MNB_E_NOMEM; }
   const unsigned want = (unsigned)std::min<size_t>(std::min<size_t>(n, slots), mem_groups);
   // CTAs per wavefront: one when the wavefronts fill the machine, a cluster when there are fewer of them than CTA slots
@@ -1328,6 +1434,12 @@ int32_t mnb_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* pos, con
 int32_t mnb_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face, double cost_limit,
                 double goal_dist_offset, float* out_dist, uint32_t* out_pred, float* out_direction, int32_t* out_cut) {
   return guarded(ctx, [&]() { return impl_cvp(ctx, seed_face, seed_pos, robot_face, cost_limit, goal_dist_offset, out_dist, out_pred, out_direction, out_cut); });
+}
+int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
+                             float* out_dist, uint32_t* out_pred, float* out_direction, int32_t* out_cutting_face) {
+  return guarded(ctx, [&]() {
+    return impl_cvp_batch_fields(ctx, n, seed_faces, seed_pos, cost_limit, out_dist, out_pred, out_direction, out_cutting_face);
+  });
 }
 int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
                       float* out_dist) {

@@ -112,18 +112,20 @@ struct CvpProblem : LabelStore {
     return face_time(c, (uint32_t)ix.x, (uint32_t)ix.y, a, b, band_end, goal, T, Tv);
   }
 
-  // predecessors_/direction_/cutting_faces_ of the winning face (cvp:493-517), literal acos form
+  // predecessors_/direction_/cutting_faces_ of the winning face (cvp:493-517), literal acos form; a null output is skipped
   __device__ __forceinline__ void write_aux(uint32_t c, int win, float wu1, float wu2) {
     if (win >= 0) {
       const int4 ix = __ldg(&cor_idx[win]);
       const float4 w = __ldg(&cor_w[win]);
       CvpResult r; r.value = 0; r.direction = 0; r.pred_sel = 1;
       cvp_update_t<true>(wu1, wu2, (double)__uint_as_float(INF_BITS), w.z, w.y, w.x, r);
-      pred[c] = r.pred_sel == 1 ? (uint32_t)ix.x : (uint32_t)ix.y;
-      dir[c] = r.direction;
-      cut[c] = ix.z;
+      if (pred) pred[c] = r.pred_sel == 1 ? (uint32_t)ix.x : (uint32_t)ix.y;
+      if (dir) dir[c] = r.direction;
+      if (cut) cut[c] = ix.z;
     } else {
-      pred[c] = c; dir[c] = 0.0f; cut[c] = -1;
+      if (pred) pred[c] = c;
+      if (dir) dir[c] = 0.0f;
+      if (cut) cut[c] = -1;
     }
   }
 
