@@ -119,7 +119,8 @@ int32_t mnb_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64
                 float* out_direction, int32_t* out_cutting_face);
 
 /* Batched full-field CVP potentials: n independent goals on the installed map, one wavefront
- * per thread-block cluster, all SMs busy.  out_dist is [n][V] row-major. */
+ * per thread-block cluster, all SMs busy.  out_dist is [n][V] row-major.  Same call as mnb_cvp_batch_fields with
+ * out_dist alone: the number of concurrent waves is capped by the free device memory as well. */
 int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n, host */,
                       const float* seed_pos /* 3n, host */, double cost_limit, float* out_dist);
 
@@ -131,9 +132,9 @@ int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n,
  * cut_k, out), which is CVPMeshPlanner::computeVectorMap (cvp_mesh_planner.cpp:204-239): one vector field per goal,
  * e.g. one per robot of a fleet.  seed_faces / seed_pos are always host pointers; the outputs follow
  * mnb_set_pointer_mode.  MNB_INVALID_START if a seed face is >= F (checked before anything is written); MNB_CANCELED
- * after mnb_cancel (the rows are then incomplete).  With out_dist alone the call runs mnb_cvp_batch's kernel; with any
+ * after mnb_cancel (the rows are then incomplete).  With out_dist alone the call is mnb_cvp_batch; with any
  * other output each wave derives its rows before it takes the next goal.  The number of concurrent waves is capped by the free
- * device memory (~76 bytes per vertex and wave) as well as by the CTA slots, so a large map runs with fewer of them;
+ * device memory (~64 bytes per vertex and wave) as well as by the CTA slots, so a large map runs with fewer of them;
  * MNB_E_NOMEM if not even one fits.  The waves share the wavefront workspace with mnb_cvp and the inflation wave: the
  * last inflation's labels are dropped (as after mnb_cvp_batch), while the outputs of the last mnb_cvp
  * (mnb_cvp_backtrack, mnb_vector_map with pred = NULL) remain available. */

@@ -600,7 +600,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
   if constexpr (FAST) { if (threadIdx.x == 0) gq_n = 0; __syncthreads(); }
   bool rescanned = false;
   float band_end_prev = band_end_init;
-  unsigned long long my_recomputes = 0, my_settled = 0, my_skipped = 0;
+  unsigned long long my_recomputes = 0, my_settled = 0;
   float lo_best = -1.0f; int stagnant = 0;       // best (largest) earliest-unsettled pop time seen so far
   prob.strict = 0;
   const uint32_t j = threadIdx.x & 7;
@@ -651,13 +651,6 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       atomicMin(&ctl->goal_ring[(r + 1) & 1], goal_b);                 // carry the cutoff into the next round
       ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag)) ? 1u : 0u;
     }
-    // Clean-candidate skip (group-uniform switch): a label is a pure function of the source labels, the band end (only
-    // through sources beyond it), the goal cutoff and -- in strict mode -- the round number.  Plans with a goal cutoff
-    // and strict rounds recompute everything; otherwise a candidate none of whose sources was re-labelled in or after the
-    // round of its own last evaluation, and whose relevant sources beyond the band end are still beyond it, keeps its
-    // label without being recomputed.
-    bool skip_ok = false;
-    if constexpr (P::CAN_SKIP) skip_ok = prob.skip_clean && !has_robot && !prob.strict;
     // Goal cutoff (cvp:754 / dijkstra:299) with a band wider than goal_dist_offset: labels computed before the cutoff
     // is known may rest on sources that turn out to lie beyond it.  Once it is known, (1) vertices beyond it never
     // settle any more -- they are recomputed under the cutoff until nothing changes -- and (2) the ones that had already
@@ -688,18 +681,9 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     auto evaluate = [&](bool has, const uint32_t c, const Label& old, const int4& ix, const float4& w, const uint32_t mk,
                         const uint32_t v0, const bool fresh, const uint32_t slot) {
       const float d = old.d, tau = old.t.a1;
-      float nd; EvTime nt; int deg; uint32_t mk1 = MARK_FIXED, mk2 = MARK_FIXED; float excl = 0.0f;
-      prob.replay_sub8(c, j, has, ix, w, band_end, goal, r, mark, old.t, nd, nt, deg, mk1, mk2, excl);
+      float nd; EvTime nt; int deg; uint32_t mk1 = MARK_FIXED, mk2 = MARK_FIXED;
+      prob.replay_sub8(c, j, has, ix, w, band_end, goal, r, mark, old.t, nd, nt, deg, mk1, mk2);
       const bool changed = has && (__float_as_uint(nd) != __float_as_uint(d) || !prob.teq(nt, old.t));
-      if constexpr (P::CAN_SKIP) if (skip_ok) {
-        // stamps of the clean-candidate skip: c was evaluated in this round; its face neighbours have a source that was
-        // re-labelled in this round (plain stores: every writer of a round stores the same value, rounds are barrier-ordered)
-        if (has && j == 0) { __stcg(&prob.last_eval[c], r + 1u); __stcg(&prob.excl_min[c], __float_as_uint(excl)); }
-        if (changed) {
-          if (ix.x != -1 && deg <= 8) { __stcg(&prob.dirty_round[ix.x], r + 1u); if constexpr (P::TWO_SOURCES) __stcg(&prob.dirty_round[ix.y], r + 1u); }
-          if (j == 0 && deg > 8) prob.activate(c, [&](uint32_t x) { __stcg(&prob.dirty_round[x], r + 1u); });
-        }
-      }
 #ifdef MNB_EMU_ACTIVE
       if (has && j == 0 && getenv("MNB_DBG_V") && (c == (uint32_t)atoi(getenv("MNB_DBG_V")) || (getenv("MNB_DBG_V2") && c == (uint32_t)atoi(getenv("MNB_DBG_V2")))))
         fprintf(stderr, "[r%u %s] c=%u old d=%.9g t=(%.9g,%u,%.9g,%.9g,ext %x) -> nd=%.9g nt=(%.9g,%u,%.9g,%.9g,ext %x) changed=%d strict=%d\n", r, fresh ? "main" : "sweep", c, old.d, old.t.a1, old.t.root, old.t.a2, old.t.a3, old.t.ext, nd, nt.a1, nt.root, nt.a2, nt.a3, nt.ext, (int)changed, prob.strict);
@@ -792,20 +776,6 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       if (has && tau < m_prev && tau < band_end_prev && tau < settle_cap) {
         if (j == 0) settle(c, old);
         has = false;
-      }
-      if constexpr (P::CAN_SKIP) if (skip_ok && has) {
-        const uint32_t le = __ldcg(&prob.last_eval[c]), dr = __ldcg(&prob.dirty_round[c]);
-        const float em = __uint_as_float(__ldcg(&prob.excl_min[c]));
-        if (le != 0u && dr < le && !(band_end > em)) {
-          // clean: survives with its label as it is (the 8 lanes of the group agree: same loads)
-          if (j == 0) {
-            my_lo = fminf(my_lo, tau);
-            my_skipped++;
-            if constexpr (SW) stage_push_seen(st, *ss, c, v0, prob.pack_label(c, old.d, old.t), list_n, &ctl->count[next]);
-            else stage_push(st, c, list_n, &ctl->count[next]);
-          }
-          has = false;
-        }
       }
       evaluate(has, c, old, ix, w, mk, v0, true, 0u);
     }
@@ -989,7 +959,6 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
   }
   atomicAdd(&ctl->recomputes, my_recomputes);
   atomicAdd(&ctl->settled, my_settled);
-  if (my_skipped) atomicAdd(&ctl->skipped, my_skipped);
   if (gtid == 0) {
     ctl->rounds += r;
     if (prob.strict) ctl->strict_armed += 1;

@@ -1,15 +1,15 @@
 // Lean round loop for BATCHES of full-field CVP plans (mnb_cvp_batch): one wavefront per CTA / cluster, hundreds in flight.
 //
 // Same algorithm, same label format and bit-identical results as run_band_rounds_sub8 (band_engine.cuh); what differs is
-// what the hot loop carries.  The generic loop serves single plans (goal cutoff + re-queueing, in-round sweeps, the
-// clean-candidate skip, robot bookkeeping) and holds the whole problem object live: at the 64 registers a 2-CTA/SM batch
+// what the hot loop carries.  The generic loop serves single plans (goal cutoff + re-queueing, in-round sweeps, robot
+// bookkeeping) and holds the whole problem object live: at the 64 registers a 2-CTA/SM batch
 // kernel may use it spilled: a large share of the executed instructions become local loads and stores, and with
 // hundreds of wavefronts in flight the local-memory footprint does not fit the L2.  A batch needs none of the extras:
 //   * fast path (98 % of the evaluations): every source label is plain (one level), no source can be a seed, the causal
 //     collapse applies -> the new label is min over the causal faces; nothing but the kernel parameters (constant bank)
 //     and five per-wavefront pointers stay live, no problem object, no pop-time algebra;
 //   * anything else (cascade members among the sources, a possible seed, non-causal faces that may fire first, more than
-//     8 faces, strict rounds) -> the warp calls the generic CvpEllProblemT::replay_sub8 through a __noinline__ wrapper
+//     8 faces, strict rounds) -> the warp calls the generic CvpEllProblem::replay_sub8 through a __noinline__ wrapper
 //     that builds the problem object on its own stack frame;
 //   * the "has activated its neighbours" state travels in bit 31 of the list entry (no mark[] load per evaluation);
 //     stage pushes are warp-aggregated by hand (one shared atomic per warp and kind).
@@ -28,7 +28,7 @@ struct BatchGroup {          // per-wavefront pointers (group g of the workspace
 
 template <class Args>
 __device__ __forceinline__ void batch_make_problem(const Args& a, const BatchGroup& G, const BatchSeeds& sd, int strict,
-                                                   CvpEllProblemT<false>& prob) {
+                                                   CvpEllProblem& prob) {
   prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
   prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo;
   prob.state = G.state; prob.ext_arr = G.ext_arr; prob.root_arr = G.root_arr; prob.chg = G.chg;
@@ -36,7 +36,7 @@ __device__ __forceinline__ void batch_make_problem(const Args& a, const BatchGro
   prob.ver = nullptr; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = nullptr; prob.dir = nullptr; prob.cut = nullptr;
   prob.cost_limit = a.cost_limit; prob.s0 = sd.s0; prob.s1 = sd.s1; prob.s2 = sd.s2; prob.seed_noexpand = sd.noexpand; prob.seed_max_d = sd.seed_max;
   prob.goal_t = ev_normal(__uint_as_float(INF_BITS), 0u);
-  prob.last_eval = nullptr; prob.dirty_round = nullptr; prob.excl_min = nullptr; prob.skip_clean = 0; prob.prefetch_marks = false;
+  prob.prefetch_marks = false;
   prob.strict = strict;
 }
 
@@ -45,11 +45,11 @@ template <class Args>
 __device__ __noinline__ void batch_slow_eval(const Args& a, const BatchGroup& G, const BatchSeeds& sd, int strict, uint32_t c, uint32_t j,
                                              bool has, const int4& ix, const float4& w, float band_end, uint32_t round, const uint4& old_bits,
                                              float& nd, EvTime& nt, float& deferred_m) {
-  CvpEllProblemT<false> prob;
+  CvpEllProblem prob;
   batch_make_problem(a, G, sd, strict, prob);
   const Label old = has ? prob.unpack_label(c, old_bits) : prob.unpack_label(0u, state_inf());
-  int deg; uint32_t mk1 = MARK_FIXED, mk2 = MARK_FIXED; float excl;
-  prob.replay_sub8(c, j, has, ix, w, band_end, __uint_as_float(INF_BITS), round, G.mark, old.t, nd, nt, deg, mk1, mk2, excl);
+  int deg; uint32_t mk1 = MARK_FIXED, mk2 = MARK_FIXED;
+  prob.replay_sub8(c, j, has, ix, w, band_end, __uint_as_float(INF_BITS), round, G.mark, old.t, nd, nt, deg, mk1, mk2);
   deferred_m = prob.deferred_m;
 }
 
@@ -58,7 +58,7 @@ template <class Args>
 __device__ __noinline__ bool batch_store_general(const Args& a, const BatchGroup& G, const BatchSeeds& sd, uint32_t c, uint32_t j, bool has,
                                                  const uint4& old_bits, float nd, const EvTime& nt, uint32_t round) {
   if (!has) return false;
-  CvpEllProblemT<false> prob;
+  CvpEllProblem prob;
   batch_make_problem(a, G, sd, 0, prob);
   const Label old = prob.unpack_label(c, old_bits);
   const bool changed = __float_as_uint(nd) != old_bits.x || !prob.teq(nt, old.t);
@@ -153,11 +153,11 @@ __device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup
           const float ta = __uint_as_float(sa.y), tb = __uint_as_float(sb.y);
           const bool v1_later = tb < ta || (tb == ta && v2 < v1);
           T1 = v1_later ? ta : tb;
-          CvpEllProblemT<false>::FaceGeo fg; fg.p = g01.x; fg.hc = g01.y; fg.t0a = g23.x;
-          CvpEllProblemT<false>::eval_face_geo((double)da, (double)db, (double)w.z, (double)w.y, (double)w.x, fg, U, X);
+          CvpEllProblem::FaceGeo fg; fg.p = g01.x; fg.hc = g01.y; fg.t0a = g23.x;
+          CvpEllProblem::eval_face_geo((double)da, (double)db, (double)w.z, (double)w.y, (double)w.x, fg, U, X);
         }
       }
-      // causal collapse (CvpEllProblemT::replay_sub8): d = min over the causal faces if no other face can fire before it
+      // causal collapse (CvpEllProblem::replay_sub8): d = min over the causal faces if no other face can fire before it
       const float Xf = (float)X;
       const bool causal = valid && Xf > T1 && U <= X;
       float m = causal ? Xf : INF;
@@ -344,7 +344,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
       __syncthreads();
       const unsigned int nwork = wk.n;
       // ---------------- phase B: one THREAD per candidate, plain causal evaluations only ----------------
-      // The throughput form of the evaluation (CvpEllProblemT::eval_plain): a thread walks the faces of its candidate (ELL
+      // The throughput form of the evaluation (CvpEllProblem::eval_plain): a thread walks the faces of its candidate (ELL
       // row), every source label plain, no possible seed, and the causal collapse applies: d = min over the causal faces.
       // ~25 warp-instructions per candidate instead of ~140 for the 8-lane form, 32 candidates per warp in flight.  Anything
       // else is deferred to phase C.
@@ -357,7 +357,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
         if (has) {
           ce = wk.q[i]; c = ce & ~LIST_ACTIVATED;
           ob = __ldcg(&G.state[c]);
-          defer = strict || !CvpEllProblemT<false>::eval_plain(a.ell_idx, a.ell_w, a.ell_geo, a.invalid, G.state, sd.seed_max, band_end, c, m, excl);
+          defer = strict || !CvpEllProblem::eval_plain(a.ell_idx, a.ell_w, a.ell_geo, a.invalid, G.state, sd.seed_max, band_end, c, m, excl);
         }
         const bool done = has && !defer;
         bool changed = false, act_now = false;

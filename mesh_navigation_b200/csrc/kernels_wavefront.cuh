@@ -19,7 +19,7 @@ struct WaveWorkspace {     // per group (index g): state + g*V etc.
   uint32_t* root;    // cascade roots of flagged labels
   uint32_t* pool;    // level pool: records of pop times with more than 3 cascade levels, pool_cap words per group
   uint32_t pool_cap;
-  uint32_t* last_eval; uint32_t* dirty; uint32_t* excl;   // clean-candidate skip stamps (problems.cuh)
+  uint32_t* last_eval; uint32_t* dirty;   // inflation only (V entries): clean-candidate stamps (InflationProblem)
   uint4* skipw;      // clean-candidate words of the batch round loop (batch_engine.cuh)
   uint32_t* chg;
   uint32_t* ver;     // single-plan only (V entries): input versions for the in-round sweeps
@@ -52,7 +52,6 @@ struct CvpKernelArgs {
   uint32_t max_rounds;
   int sweeps;                   // in-round sweeps of a single plan (0 = off, -1 = from the band width)
   float hop;                    // ~ one dependency hop in potential units (1.35 x mean edge weight)
-  int skip_clean;               // clean-candidate skip (band_engine.cuh), 0 = off
 };
 
 template <int CS>
@@ -82,7 +81,7 @@ __device__ __forceinline__ void ctl_reset(GroupCtl* ctl, unsigned int n0, float 
 #ifndef MNB_CVP_THREADS
 #define MNB_CVP_THREADS 512
 #endif
-template <int CS, bool SKIP>
+template <int CS>
 __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(const CvpKernelArgs a) {
   __shared__ Stage st;
   uint32_t g, gthreads, gtid;
@@ -104,24 +103,22 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
     const bool single = (a.n_queries == 1);
     uint32_t* chg = a.ws.chg + (size_t)g * V;
     const int sweeps = 0;                            // in-round sweeps are compiled into the whole-grid kernel only
-    uint32_t* last_eval = a.ws.last_eval + (size_t)g * V; uint32_t* dirty = a.ws.dirty + (size_t)g * V;
     for (uint32_t v = gtid; v < V; v += gthreads) {
       state[v] = state_inf(); mark[v] = MARK_NONE; chg[v] = 0u;
-      if constexpr (SKIP) { last_eval[v] = 0u; dirty[v] = 0u; }
       if (sweeps) a.ws.ver[v] = 0u;
     }
     group_sync<CS>();
 
     const uint32_t sf = a.seed_faces[q];
     const uint32_t s0 = a.faces[3 * (size_t)sf], s1 = a.faces[3 * (size_t)sf + 1], s2 = a.faces[3 * (size_t)sf + 2];
-    CvpEllProblemT<SKIP> prob;
+    CvpEllProblem prob;
     prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
     prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo;
     prob.state = state; prob.ext_arr = a.ws.ext + (size_t)g * V; prob.root_arr = a.ws.root + (size_t)g * V; prob.chg = chg;
     prob.pool_w = a.ws.pool + (size_t)g * a.ws.pool_cap; prob.pool = prob.pool_w; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
     prob.ver = a.ws.ver; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = nullptr; prob.dir = nullptr; prob.cut = nullptr; prob.cost_limit = a.cost_limit;
     prob.s0 = s0; prob.s1 = s1; prob.s2 = s2; prob.seed_noexpand = 0; prob.goal_t = ev_normal(__uint_as_float(INF_BITS), 0u);
-    prob.last_eval = last_eval; prob.dirty_round = dirty; prob.excl_min = a.ws.excl + (size_t)g * V; prob.skip_clean = SKIP ? 1 : 0; prob.prefetch_marks = false;
+    prob.prefetch_marks = false;
     float sd[3];
     {
       const uint32_t sv[3] = {s0, s1, s2};
@@ -241,7 +238,7 @@ __device__ __noinline__ void batch_fields_epilogue(const CvpKernelArgs& a, const
   for (uint32_t v = gtid; v < V; v += gthreads) cvp_epilogue_vertex(prob, G.ctl, sf, __uint_as_float(INF_BITS), v);
 }
 
-// FIELDS = false: potentials only (mnb_cvp_batch, and the whole-grid experiment CS = 0).  FIELDS = true (mnb_cvp_batch_fields):
+// FIELDS = false: potentials only (mnb_cvp_batch, and mnb_cvp_batch_fields asked for potentials alone).  FIELDS = true:
 // each group also runs the epilogue of its goal before it takes the next one, and takes none once the cancel flag is set.
 template <int CS, bool FIELDS>
 __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_batch(const CvpKernelArgs a) {
@@ -322,7 +319,6 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
 #ifndef MNB_GRID_MINBLOCKS
 #define MNB_GRID_MINBLOCKS 1
 #endif
-template <bool SKIP>
 __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpKernelArgs a) {
   __shared__ Stage st;
   __shared__ SweepStage sws;
@@ -333,21 +329,18 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
   GroupCtl* ctl = a.ws.ctl;
   if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; sws.dn[0] = 0; sws.dn[1] = 0; }
   __syncthreads();
-  for (uint32_t v = gtid; v < V; v += gthreads) {
-    state[v] = state_inf(); mark[v] = MARK_NONE; a.ws.chg[v] = 0u; a.ws.ver[v] = 0u;
-    if constexpr (SKIP) { a.ws.last_eval[v] = 0u; a.ws.dirty[v] = 0u; }
-  }
+  for (uint32_t v = gtid; v < V; v += gthreads) { state[v] = state_inf(); mark[v] = MARK_NONE; a.ws.chg[v] = 0u; a.ws.ver[v] = 0u; }
   group_sync<0>(ctl->barrier);
   const uint32_t sf = a.seed_faces[0];
   const uint32_t s0 = a.faces[3 * (size_t)sf], s1 = a.faces[3 * (size_t)sf + 1], s2 = a.faces[3 * (size_t)sf + 2];
-  CvpEllProblemT<SKIP> prob;
+  CvpEllProblem prob;
   prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
   prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo;
   prob.state = state; prob.ext_arr = a.ws.ext; prob.root_arr = a.ws.root; prob.chg = a.ws.chg;
   prob.pool_w = a.ws.pool; prob.pool = prob.pool_w; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
   prob.ver = a.ws.ver; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = nullptr; prob.dir = nullptr; prob.cut = nullptr; prob.cost_limit = a.cost_limit;
   prob.s0 = s0; prob.s1 = s1; prob.s2 = s2; prob.seed_noexpand = 0; prob.goal_t = ev_normal(__uint_as_float(INF_BITS), 0u);
-  prob.last_eval = a.ws.last_eval; prob.dirty_round = a.ws.dirty; prob.excl_min = a.ws.excl; prob.skip_clean = SKIP ? 1 : 0; prob.prefetch_marks = true;
+  prob.prefetch_marks = true;
   float sd[3];
   {
     const uint32_t sv[3] = {s0, s1, s2};

@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/meshnav_b200.h"
@@ -86,15 +87,12 @@ struct mnb_ctx {
   // tuning
   float delta = 0.3f; int cluster = -1 /* -1: whole-grid cooperative kernel for single plans */; int batch_cluster = 0 /* 0: chosen per call from the goal count */; int threads = 512;
   int grid_blocks_per_sm = 0;
-  int infl_skip_clean = 1;     // clean-candidate skip of the inflation wave (MNB_INFL_SKIP=0 turns it off)
+  int infl_skip_clean = 1;     // clean-candidate skip of the inflation wave (mnb_debug_set_infl_skip(ctx, 0) turns it off)
   int layers_smem = 5;         // neighbourhood walk of k_layers: 0 thread-local seen-set, 1 shared-memory seen-set, 2-4 prefetching walk (64 / 128 / 32
                                // threads per CTA), 5-7 the same with the 16-bit seen-set (64 / 128 / 256), 8-9 its low-register builds.
-                               // Chosen per mesh by mnb_set_mesh unless fixed by the caller.
+                               // Chosen per mesh by mnb_set_mesh unless fixed by mnb_debug_set_layers_smem.
   bool layers_explicit = false;
-  int skip_clean = 0;          // clean-candidate stamps of the generic 8-lane CVP loop: measured slower than without them, its kernel
-                               // instantiations are no longer built; the flag only reaches the legacy per-cluster kernel args.  The batch engine
-                               // and the inflation wave carry their own (exact) rule.
-  int sweeps = -1;             // in-round sweeps of the whole-grid single-plan kernel; -1 = derived from the band width
+  int sweeps = -1;             // in-round sweeps of the whole-grid single plans (mnb_debug_set_sweeps); -1 = derived from the band width
   float grid_delta = 1.8f;     // band width of the whole-grid single-plan kernel (wide band + in-round sweeps)
   float dijkstra_grid_delta = 3.0f;
   float dijkstra_batch_delta = 0.18f;
@@ -105,8 +103,6 @@ struct mnb_ctx {
   // ~1.35 w (the in-round sweeps are counted in hops).  On the 0.1 m bench meshes (w = 0.118) that is 0.3 / 2.4 / 3.0 m, the values
   // the kernels were tuned with.
   bool delta_explicit = false; float w_mean = 0.0f; double* d_wsum = nullptr;
-  int grid_engine = 0;         // experiment: 1 = full-field single plans run the lean batch round loop on the whole grid (k_cvp_batch<0>)
-  float grid2_delta_w = 2.5f;  //             its band width in mean edge weights
   // ray caster over the faces (kernels_raycast.cuh; built on first use) + state of the obstacle layer
   RayBvh bvh{}; bool bvh_valid = false; unsigned int* d_ray_overflow = nullptr;
   float* d_ray_in = nullptr; size_t ray_in_cap = 0; float* d_ray_out = nullptr; size_t ray_out_cap = 0;
@@ -136,7 +132,7 @@ static void free_mesh(mnb_ctx* c) {
   dfree(c->d_pos); dfree(c->d_faces); dfree(c->d_edges); dfree(c->d_cor_ptr); dfree(c->d_cor_idx); dfree(c->d_cor_eid); dfree(c->d_face_cor);
   dfree(c->d_cor_w); dfree(c->d_cor_wd); dfree(c->d_ell_idx); dfree(c->d_ell_eid); dfree(c->d_ell_w); dfree(c->d_ell_wd); dfree(c->d_ell_geo); dfree(c->d_adj_ptr); dfree(c->d_adj_nbr); dfree(c->d_adj_eid); dfree(c->d_adj_nw); dfree(c->d_ell_adj);
   dfree(c->d_edge_dist); dfree(c->d_edge_w); dfree(c->d_cost); dfree(c->d_invalid); dfree(c->d_wsum);
-  dfree(c->ws.state); dfree(c->ws.ext); dfree(c->ws.pool); dfree(c->ws.skipw); dfree(c->ws.root); dfree(c->ws.last_eval); dfree(c->ws.dirty); dfree(c->ws.excl); dfree(c->ws.chg); dfree(c->ws.ver); dfree(c->ws.mark); dfree(c->ws.list0); dfree(c->ws.list1); dfree(c->ws.ctl);
+  dfree(c->ws.state); dfree(c->ws.ext); dfree(c->ws.pool); dfree(c->ws.skipw); dfree(c->ws.root); dfree(c->ws.last_eval); dfree(c->ws.dirty); dfree(c->ws.chg); dfree(c->ws.ver); dfree(c->ws.mark); dfree(c->ws.list0); dfree(c->ws.list1); dfree(c->ws.ctl);
   c->ws_groups = 0;
   dfree(c->dws.label); dfree(c->dws.mark); dfree(c->dws.list0); dfree(c->dws.list1); dfree(c->dws.ctl); c->dws_groups = 0;
   dfree(c->d_batch_pred); c->batch_pred_cap = 0; dfree(c->d_batch_dir); c->batch_dir_cap = 0; dfree(c->d_batch_cut); c->batch_cut_cap = 0;
@@ -155,18 +151,18 @@ static void free_mesh(mnb_ctx* c) {
 // level pool (band_engine.cuh): pop times with more than 3 cascade levels keep their tails here; 2 words per vertex
 // hold the deepest flooded pockets randomised testing has produced with room to spare; exhaustion is reported
 static uint32_t ws_pool_cap(uint32_t V) { return (uint32_t)std::min<size_t>(std::max<size_t>(65536, 2 * (size_t)V), 0x7fffffffu); }
-// device bytes of one group of the wavefront workspace (ensure_workspace): two 16-byte and nine 4-byte words per vertex,
-// the level pool and the GroupCtl -- 76 bytes per vertex on large maps
+// device bytes of one group of the wavefront workspace (ensure_workspace): two 16-byte and six 4-byte words per vertex,
+// the level pool and the GroupCtl -- 64 bytes per vertex on large maps
 static size_t ws_bytes_per_group(uint32_t V) {
-  return (size_t)V * (2 * sizeof(uint4) + 9 * sizeof(uint32_t)) + (size_t)ws_pool_cap(V) * sizeof(uint32_t) + sizeof(GroupCtl);
+  return (size_t)V * (2 * sizeof(uint4) + 6 * sizeof(uint32_t)) + (size_t)ws_pool_cap(V) * sizeof(uint32_t) + sizeof(GroupCtl);
 }
 
 static int32_t ensure_workspace(mnb_ctx* ctx, uint32_t groups) {
   if (groups <= ctx->ws_groups) return MNB_OK;
-  dfree(ctx->ws.state); dfree(ctx->ws.ext); dfree(ctx->ws.pool); dfree(ctx->ws.skipw); dfree(ctx->ws.root); dfree(ctx->ws.last_eval); dfree(ctx->ws.dirty); dfree(ctx->ws.excl); dfree(ctx->ws.chg); dfree(ctx->ws.ver); dfree(ctx->ws.mark); dfree(ctx->ws.list0); dfree(ctx->ws.list1); dfree(ctx->ws.ctl);
+  dfree(ctx->ws.state); dfree(ctx->ws.ext); dfree(ctx->ws.pool); dfree(ctx->ws.skipw); dfree(ctx->ws.root); dfree(ctx->ws.last_eval); dfree(ctx->ws.dirty); dfree(ctx->ws.chg); dfree(ctx->ws.ver); dfree(ctx->ws.mark); dfree(ctx->ws.list0); dfree(ctx->ws.list1); dfree(ctx->ws.ctl);
   ctx->ws_groups = 0;
   const size_t n = (size_t)groups * ctx->V;
-  CK(dalloc(&ctx->ws.state, n)); CK(dalloc(&ctx->ws.ext, n)); CK(dalloc(&ctx->ws.skipw, n)); CK(dalloc(&ctx->ws.root, n)); CK(dalloc(&ctx->ws.last_eval, n)); CK(dalloc(&ctx->ws.dirty, n)); CK(dalloc(&ctx->ws.excl, n)); CK(dalloc(&ctx->ws.chg, n)); CK(dalloc(&ctx->ws.ver, (size_t)ctx->V)); CK(dalloc(&ctx->ws.mark, n)); CK(dalloc(&ctx->ws.list0, n)); CK(dalloc(&ctx->ws.list1, n));
+  CK(dalloc(&ctx->ws.state, n)); CK(dalloc(&ctx->ws.ext, n)); CK(dalloc(&ctx->ws.skipw, n)); CK(dalloc(&ctx->ws.root, n)); CK(dalloc(&ctx->ws.last_eval, (size_t)ctx->V)); CK(dalloc(&ctx->ws.dirty, (size_t)ctx->V)); CK(dalloc(&ctx->ws.chg, n)); CK(dalloc(&ctx->ws.ver, (size_t)ctx->V)); CK(dalloc(&ctx->ws.mark, n)); CK(dalloc(&ctx->ws.list0, n)); CK(dalloc(&ctx->ws.list1, n));
   ctx->ws.pool_cap = ws_pool_cap(ctx->V);
   CK(dalloc(&ctx->ws.pool, (size_t)groups * ctx->ws.pool_cap));
   CK(dalloc(&ctx->ws.ctl, groups));
@@ -206,12 +202,6 @@ int32_t mnb_create(int32_t device, mnb_ctx** out_ctx) {
   if (cudaSetDevice(device) != cudaSuccess) return MNB_E_CUDA;
   mnb_ctx* c = new mnb_ctx();
   c->device = device; c->sm_count = prop.multiProcessorCount;
-  if (const char* e = getenv("MNB_INFL_SKIP")) c->infl_skip_clean = atoi(e) != 0;                                 // experiment knob
-  if (const char* e = getenv("MNB_LAYERS_SMEM")) { c->layers_smem = atoi(e); c->layers_explicit = true; }                                   // experiment knob
-  if (const char* e = getenv("MNB_SKIP_CLEAN")) c->skip_clean = atoi(e) != 0;                                     // experiment knob
-  if (const char* e = getenv("MNB_GRID_ENGINE")) c->grid_engine = atoi(e);                                     // experiment knob
-  if (const char* e = getenv("MNB_GRID2_DELTA_W")) { const float k = (float)atof(e); if (k > 0) c->grid2_delta_w = k; }
-  if (const char* e = getenv("MNB_SWEEPS")) { const int k = atoi(e); if (k >= -1 && k <= 64) c->sweeps = k; }   // experiment knob
   if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return MNB_E_CUDA; }
   cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
   cudaMalloc((void**)&c->d_next_query, sizeof(unsigned int));
@@ -562,29 +552,43 @@ static cudaError_t device_memory(int device, size_t* free_b, size_t* total_b) {
 #endif
 }
 
-// concurrent wavefronts the device memory allows for a workspace of per_group bytes per wavefront: the free memory plus the
-// `current` groups a larger workspace would replace, less a reserve (512 MB or 1/32 of the device); 0 if not even one fits
-static int32_t memory_capped_groups(mnb_ctx* ctx, size_t per_group, uint32_t current, size_t* groups) {
+// Calls launch(std::integral_constant<int, CS>()) with the cluster size cs as a compile-time constant: 1, 2, 4 and 8 as
+// given, anything else as MAX_CS (8 for the batch kernels, 16 for single plans), so a kernel template is instantiated for
+// exactly these sizes.
+template <int MAX_CS, class F>
+static cudaError_t with_cluster_size(int cs, F&& launch) {
+  switch (cs) {
+    case 1: return launch(std::integral_constant<int, 1>());
+    case 2: return launch(std::integral_constant<int, 2>());
+    case 4: return launch(std::integral_constant<int, 4>());
+    case 8: return launch(std::integral_constant<int, 8>());
+    default: return launch(std::integral_constant<int, MAX_CS>());
+  }
+}
+
+// Launch shape of a batch of n wavefronts on kernel `kern` (its one-CTA instantiation).  Concurrent wavefronts: the CTA
+// slots its occupancy allows (at most MNB_BATCH_MINBLOCKS per SM), capped by the device memory a workspace of per_group
+// bytes per wavefront may take -- the free memory plus the `current` groups a larger workspace would replace, less a
+// reserve (512 MB or 1/32 of the device); MNB_E_NOMEM if not even one fits.  CTAs per wavefront (unless mnb_set_tuning
+// fixed them): one when the wavefronts fill the machine, a cluster when there are fewer of them than CTA slots, so that
+// the SMs do not idle (strong scaling across GPUs hands every rank a fraction of the batch).
+template <class KArgs>
+static int32_t batch_shape(mnb_ctx* ctx, void (*kern)(const KArgs), uint32_t n, size_t per_group, uint32_t current,
+                           const char* what, int* cs_out, unsigned* groups_out) {
+  int per_sm = 1;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MNB_BATCH_THREADS, 0));
+  const unsigned slots = (unsigned)(ctx->sm_count * std::max(1, std::min(per_sm, (int)MNB_BATCH_MINBLOCKS)));
   size_t free_b = 0, total_b = 0;
   CK(device_memory(ctx->device, &free_b, &total_b));
   const size_t avail = free_b + (size_t)current * per_group;
   const size_t reserve = std::max<size_t>((size_t)512 << 20, total_b / 32);
-  *groups = avail > reserve ? (avail - reserve) / per_group : 0;
-  return MNB_OK;
-}
-
-static int32_t launch_cvp(mnb_ctx* ctx, const CvpKernelArgs& a, int cs, unsigned groups) {
-  cudaError_t e;
-  const unsigned blocks = groups * cs;
-  const int threads = MNB_CVP_THREADS;
-  switch (cs) {
-    case 1: e = launch_cluster(k_cvp<1, false>, a, 1, blocks, threads, ctx->stream); break;
-    case 2: e = launch_cluster(k_cvp<2, false>, a, 2, blocks, threads, ctx->stream); break;     // (the skip variant is built for the two
-    case 4: e = launch_cluster(k_cvp<4, false>, a, 4, blocks, threads, ctx->stream); break;     //  default configurations only: per-CTA batches
-    case 8: e = launch_cluster(k_cvp<8, false>, a, 8, blocks, threads, ctx->stream); break;     //  and the whole-grid single plan)
-    default: e = launch_cluster(k_cvp<16, false>, a, 16, blocks, threads, ctx->stream); break;
-  }
-  if (e != cudaSuccess) { ctx->err = std::string("cvp launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
+  const size_t mem_groups = avail > reserve ? (avail - reserve) / per_group : 0;
+  if (mem_groups == 0) { ctx->err = std::string("not enough free device memory for one ") + what + " wavefront"; return MNB_E_NOMEM; }
+  const unsigned want = (unsigned)std::min<size_t>(std::min<size_t>(n, slots), mem_groups);
+  int cs = ctx->batch_cluster;
+  if (cs <= 0) { cs = 1; while (cs < 8 && (unsigned)(2 * cs) * want <= slots) cs *= 2; }
+  *cs_out = cs;
+  *groups_out = std::min(want, std::max(1u, slots / (unsigned)cs));
   return MNB_OK;
 }
 
@@ -627,7 +631,7 @@ static void fill_cvp_args(mnb_ctx* ctx, CvpKernelArgs& a) {
   a.V = ctx->V; a.pos = ctx->d_pos; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx;
   a.cor_w = ctx->d_cor_w; a.ell_idx = ctx->d_ell_idx; a.ell_w = ctx->d_ell_w; a.ell_geo = ctx->d_ell_geo; a.cost = ctx->d_cost; a.invalid = ctx->has_invalid ? ctx->d_invalid : nullptr; a.ws = ctx->ws;
   a.seed_faces = ctx->d_seed_faces; a.seed_pos = ctx->d_seed_pos; a.delta = ctx->delta; a.next_query = ctx->d_next_query;
-  a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V); a.sweeps = 0; a.skip_clean = ctx->skip_clean;
+  a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V); a.sweeps = 0;
   a.hop = ctx->w_mean > 0 ? 1.35f * ctx->w_mean : 0.16f;
 }
 
@@ -666,21 +670,17 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
     a.delta = ctx->grid_delta;
     if (ctx->grid_blocks_per_sm == 0) {
       int nb = 0;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_cvp_grid<false>, ctx->threads, 0));
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_cvp_grid, ctx->threads, 0));
       ctx->grid_blocks_per_sm = nb > MNB_GRID_MINBLOCKS ? MNB_GRID_MINBLOCKS : nb;
       if (nb <= 0) { ctx->err = "k_cvp_grid cannot be resident"; return MNB_E_CUDA; }
     }
-    if (ctx->grid_engine == 1 && robot_face < 0) {
-      int per_sm = 1;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp_batch<0, false>, MNB_BATCH_THREADS, 0));
-      if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
-      if (per_sm < 1) { ctx->err = "k_cvp_batch<0> cannot be resident"; return MNB_E_CUDA; }
-      a.delta = ctx->grid2_delta_w * (ctx->w_mean > 0.0f ? ctx->w_mean : 0.12f);
-      CK(launch_cooperative(k_cvp_batch<0, false>, a, (unsigned)(ctx->sm_count * per_sm), MNB_BATCH_THREADS, ctx->stream));
-    } else
-    CK(launch_cooperative(k_cvp_grid<false>, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
+    CK(launch_cooperative(k_cvp_grid, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
   } else {
-    if ((rc = launch_cvp(ctx, a, ctx->cluster, 1)) != MNB_OK) return rc;
+    const cudaError_t e = with_cluster_size<16>(ctx->cluster, [&](auto c) {
+      constexpr int CS = decltype(c)::value;
+      return launch_cluster(k_cvp<CS>, a, CS, (unsigned)CS, MNB_CVP_THREADS, ctx->stream);
+    });
+    if (e != cudaSuccess) { ctx->err = std::string("cvp launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   }
   MNB_LAUNCH(k_cvp_epilogue, (ctx->V + 255) / 256, 256, 0, ctx->stream, a, ctx->ws.ctl);
   CK(cudaGetLastError());
@@ -713,68 +713,10 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   return MNB_SUCCESS;
 }
 
-static int32_t impl_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
-                      float* out_dist) {
-  if (!ctx || !seed_faces || !seed_pos || !out_dist || !ctx->V || n == 0) return MNB_E_ARG;
-  if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
-  for (uint32_t i = 0; i < n; ++i) if (seed_faces[i] >= ctx->F) return MNB_INVALID_START;
-  CK(cudaSetDevice(ctx->device));
-  // resident CTAs per SM of the lean batch kernel (k_cvp_batch, batch_engine.cuh); MNB_BATCH_LEGACY=1 runs the generic
-  // round loop (k_cvp) instead -- kept for A/B measurements
-  static const bool legacy = getenv("MNB_BATCH_LEGACY") != nullptr;
-  int per_sm = 1;
-  if (legacy) { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp<1, false>, MNB_CVP_THREADS, 0)); if (per_sm > 2) per_sm = 2; }
-  else { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cvp_batch<1, false>, MNB_BATCH_THREADS, 0)); if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS; }
-  if (per_sm < 1) per_sm = 1;
-  const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
-  // CTAs per wavefront: one when the goals fill the machine; with fewer goals than CTA slots a cluster of CTAs shares a
-  // wavefront so that the SMs do not idle (strong scaling across GPUs hands every rank a fraction of the batch)
-  int cs = ctx->batch_cluster;
-  if (cs <= 0) { cs = 1; while (cs < 8 && (unsigned)(2 * cs) * n <= slots) cs *= 2; }
-  if (cs > 1) per_sm = std::max(1, std::min(per_sm, 2));
-  unsigned groups = slots / (unsigned)cs;
-  if (groups > n) groups = n;
-  if (groups == 0) groups = 1;
-  int32_t rc;
-  if ((rc = ensure_workspace(ctx, groups)) != MNB_OK) return rc;
-  if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  if ((rc = ensure_out(ctx, dev ? 0 : (size_t)n * ctx->V, false)) != MNB_OK) return rc;
-  if (ctx->h_cancel) *ctx->h_cancel = 0;
-  ctx->infl_labels_valid = false;
-  CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_faces, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
-  CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
-  CvpKernelArgs a{};
-  fill_cvp_args(ctx, a);
-  a.n_queries = n; a.robot_face = -1; a.cost_limit = cost_limit; a.goal_dist_offset = 0.0;
-  a.out_dist = dev ? out_dist : ctx->d_out_dist;
-  a.out_pred = nullptr; a.out_dir = nullptr; a.out_cut = nullptr;
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  if (legacy) { if ((rc = launch_cvp(ctx, a, cs, groups)) != MNB_OK) return rc; }
-  else {
-    cudaError_t e;
-    const unsigned blocks = groups * (unsigned)cs;
-    switch (cs) {
-      case 1: e = launch_cluster(k_cvp_batch<1, false>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 2: e = launch_cluster(k_cvp_batch<2, false>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 4: e = launch_cluster(k_cvp_batch<4, false>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      default: e = launch_cluster(k_cvp_batch<8, false>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-    }
-    if (e != cudaSuccess) { ctx->err = std::string("cvp batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
-  }
-  CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)n * ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-  if ((rc = finish_stats(ctx, groups, 1)) != MNB_OK) return rc;
-  if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
-  return MNB_SUCCESS;
-}
-
-// n full-field CVP plans with their vector-field inputs in one launch (k_cvp_batch<CS, true>): each wavefront runs the
-// epilogue of its goal before its group takes the next one.  Only potentials requested: the potentials-only kernel.  The
-// waves share the wavefront workspace with single plans and inflation (not the single plan's outputs), and their number
-// is capped by the free device memory as well as by the CTA slots.
+// n full-field CVP plans in one launch, mnb_cvp_batch and mnb_cvp_batch_fields.  With vector-field outputs
+// (k_cvp_batch<CS, true>) each wavefront runs the epilogue of its goal before its group takes the next one; potentials
+// alone run the potentials-only kernel.  The waves share the wavefront workspace with single plans and inflation (not the
+// single plan's outputs), and their number is capped by the free device memory as well as by the CTA slots.
 static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
                                      float* out_dist, uint32_t* out_pred, float* out_dir, int32_t* out_cut) {
   if (!ctx || !seed_faces || !seed_pos || (!out_dist && !out_pred && !out_dir && !out_cut) || !ctx->V || n == 0) return MNB_E_ARG;
@@ -802,20 +744,10 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
       CK(dalloc(&ctx->d_batch_cut, rows)); ctx->batch_cut_cap = rows;
     }
   }
-  // concurrent wavefronts: the CTA slots of the kernel, capped by the device memory their workspace may take
-  int per_sm = 1;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fields ? k_cvp_batch<1, true> : k_cvp_batch<1, false>, MNB_BATCH_THREADS, 0));
-  if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
-  if (per_sm < 1) per_sm = 1;
-  const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
-  size_t mem_groups = 0;
-  if ((rc = memory_capped_groups(ctx, ws_bytes_per_group(ctx->V), ctx->ws_groups, &mem_groups)) != MNB_OK) return rc;
-  if (mem_groups == 0) { ctx->err = "not enough free device memory for one CVP wavefront"; return MNB_E_NOMEM; }
-  const unsigned want = (unsigned)std::min<size_t>(std::min<size_t>(n, slots), mem_groups);
-  // CTAs per wavefront: one when the wavefronts fill the machine, a cluster when there are fewer of them than CTA slots
-  int cs = ctx->batch_cluster;
-  if (cs <= 0) { cs = 1; while (cs < 8 && (unsigned)(2 * cs) * want <= slots) cs *= 2; }
-  const unsigned groups = std::min(want, std::max(1u, slots / (unsigned)cs));
+  int cs = 1; unsigned groups = 1;
+  rc = fields ? batch_shape(ctx, k_cvp_batch<1, true>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
+              : batch_shape(ctx, k_cvp_batch<1, false>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups);
+  if (rc != MNB_OK) return rc;
   if ((rc = ensure_workspace(ctx, groups)) != MNB_OK) return rc;
   if (ctx->h_cancel) *ctx->h_cancel = 0;
   ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
@@ -831,24 +763,13 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
   a.out_dir = !out_dir ? nullptr : (dev ? out_dir : ctx->d_batch_dir);
   a.out_cut = !out_cut ? nullptr : (dev ? out_cut : ctx->d_batch_cut);
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  cudaError_t e;
   const unsigned blocks = groups * (unsigned)cs;
-  if (fields) {
-    switch (cs) {
-      case 1: e = launch_cluster(k_cvp_batch<1, true>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 2: e = launch_cluster(k_cvp_batch<2, true>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 4: e = launch_cluster(k_cvp_batch<4, true>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      default: e = launch_cluster(k_cvp_batch<8, true>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-    }
-  } else {
-    switch (cs) {
-      case 1: e = launch_cluster(k_cvp_batch<1, false>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 2: e = launch_cluster(k_cvp_batch<2, false>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      case 4: e = launch_cluster(k_cvp_batch<4, false>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-      default: e = launch_cluster(k_cvp_batch<8, false>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-    }
-  }
-  if (e != cudaSuccess) { ctx->err = std::string("cvp batch fields launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
+  const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
+    constexpr int CS = decltype(c)::value;
+    return fields ? launch_cluster(k_cvp_batch<CS, true>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
+                  : launch_cluster(k_cvp_batch<CS, false>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
+  });
+  if (e != cudaSuccess) { ctx->err = std::string("cvp batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (!dev) {
     if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * rows, cudaMemcpyDeviceToHost, ctx->stream));
@@ -901,13 +822,11 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   if (cs == -1) {   // single plan on the whole GPU (cooperative launch, one CTA per SM)
     a.delta = ctx->dijkstra_grid_delta; a.ell_adj = ctx->d_ell_adj; a.sweeps = ctx->sweeps; a.hop = ctx->w_mean > 0 ? 1.35f * ctx->w_mean : 0.16f;
     e = launch_cooperative(k_dijkstra_grid, a, (unsigned)ctx->sm_count, 512, ctx->stream);
-  } else
-  switch (cs) {
-    case 1: e = launch_cluster(k_dijkstra<1>, a, 1, 1, ctx->threads, ctx->stream); break;
-    case 2: e = launch_cluster(k_dijkstra<2>, a, 2, 2, ctx->threads, ctx->stream); break;
-    case 4: e = launch_cluster(k_dijkstra<4>, a, 4, 4, ctx->threads, ctx->stream); break;
-    case 8: e = launch_cluster(k_dijkstra<8>, a, 8, 8, ctx->threads, ctx->stream); break;
-    default: e = launch_cluster(k_dijkstra<16>, a, 16, 16, ctx->threads, ctx->stream); break;
+  } else {
+    e = with_cluster_size<16>(cs, [&](auto c) {
+      constexpr int CS = decltype(c)::value;
+      return launch_cluster(k_dijkstra<CS>, a, CS, (unsigned)CS, ctx->threads, ctx->stream);
+    });
   }
   if (e != cudaSuccess) { ctx->err = std::string("dijkstra launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
@@ -942,20 +861,9 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
       CK(dalloc(&ctx->d_batch_pred, (size_t)n * V)); ctx->batch_pred_cap = (size_t)n * V;
     }
   }
-  // concurrent wavefronts: the CTA slots of the kernel, capped by the device memory their workspace may take
-  int per_sm = 1;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_dijkstra_batch<1>, MNB_BATCH_THREADS, 0));
-  if (per_sm > MNB_BATCH_MINBLOCKS) per_sm = MNB_BATCH_MINBLOCKS;
-  if (per_sm < 1) per_sm = 1;
-  const unsigned slots = (unsigned)(ctx->sm_count * per_sm);
-  size_t mem_groups = 0;
-  if ((rc = memory_capped_groups(ctx, DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl), ctx->dws_groups, &mem_groups)) != MNB_OK) return rc;
-  if (mem_groups == 0) { ctx->err = "not enough free device memory for one Dijkstra wavefront"; return MNB_E_NOMEM; }
-  const unsigned want = (unsigned)std::min<size_t>(std::min<size_t>(n, slots), mem_groups);
-  // CTAs per wavefront: one when the wavefronts fill the machine, a cluster when there are fewer of them than CTA slots
-  int cs = ctx->batch_cluster;
-  if (cs <= 0) { cs = 1; while (cs < 8 && (unsigned)(2 * cs) * want <= slots) cs *= 2; }
-  unsigned groups = std::min(want, std::max(1u, slots / (unsigned)cs));
+  int cs = 1; unsigned groups = 1;
+  if ((rc = batch_shape(ctx, k_dijkstra_batch<1>, n, DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl), ctx->dws_groups,
+                        "Dijkstra", &cs, &groups)) != MNB_OK) return rc;
   if (groups > ctx->dws_groups) {
     dfree(ctx->dws.label); dfree(ctx->dws.mark); dfree(ctx->dws.list0); dfree(ctx->dws.list1); dfree(ctx->dws.ctl); ctx->dws_groups = 0;
     const size_t m = (size_t)groups * V;
@@ -976,14 +884,11 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
   a.next_query = ctx->d_next_query; a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V);
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  cudaError_t e;
   const unsigned blocks = groups * (unsigned)cs;
-  switch (cs) {
-    case 1: e = launch_cluster(k_dijkstra_batch<1>, a, 1, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-    case 2: e = launch_cluster(k_dijkstra_batch<2>, a, 2, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-    case 4: e = launch_cluster(k_dijkstra_batch<4>, a, 4, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-    default: e = launch_cluster(k_dijkstra_batch<8>, a, 8, blocks, MNB_BATCH_THREADS, ctx->stream); break;
-  }
+  const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
+    constexpr int CS = decltype(c)::value;
+    return launch_cluster(k_dijkstra_batch<CS>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
+  });
   if (e != cudaSuccess) { ctx->err = std::string("dijkstra batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (!dev) {
@@ -1185,10 +1090,8 @@ static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32
 // experiment knob (not part of the public header): in-round sweeps of the whole-grid single-plan kernel
 int32_t mnb_debug_set_sweeps(mnb_ctx* ctx, int32_t k) { if (!ctx || k < -1 || k > 64) return MNB_E_ARG; ctx->sweeps = k; return MNB_OK; }
 
-int32_t mnb_debug_set_grid_engine(mnb_ctx* ctx, int32_t mode, float delta_w) { if (!ctx) return MNB_E_ARG; ctx->grid_engine = mode; if (delta_w > 0) ctx->grid2_delta_w = delta_w; return MNB_OK; }
 int32_t mnb_debug_set_infl_skip(mnb_ctx* ctx, int32_t on) { if (!ctx) return MNB_E_ARG; ctx->infl_skip_clean = on != 0; return MNB_OK; }
 int32_t mnb_debug_set_layers_smem(mnb_ctx* ctx, int32_t mode) { if (!ctx || mode < 0 || mode > 9) return MNB_E_ARG; ctx->layers_smem = mode; ctx->layers_explicit = true; return MNB_OK; }
-int32_t mnb_debug_set_skip_clean(mnb_ctx* ctx, int32_t on) { if (!ctx) return MNB_E_ARG; ctx->skip_clean = on != 0; ctx->grid_blocks_per_sm = 0; return MNB_OK; }
 
 // debugging aid (not part of the public header): raw labels {d, a1, a2, a3|flag} of wavefront group 0
 int32_t mnb_debug_get_labels(mnb_ctx* ctx, uint32_t* out4v) {
@@ -1443,7 +1346,7 @@ int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_face
 }
 int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
                       float* out_dist) {
-  return guarded(ctx, [&]() { return impl_cvp_batch(ctx, n, seed_faces, seed_pos, cost_limit, out_dist); });
+  return guarded(ctx, [&]() { return impl_cvp_batch_fields(ctx, n, seed_faces, seed_pos, cost_limit, out_dist, nullptr, nullptr, nullptr); });
 }
 int32_t mnb_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_vertex, double cost_limit, double goal_dist_offset,
                      float* out_dist, uint32_t* out_pred) {

@@ -21,7 +21,6 @@ namespace mnb {
 //     among the cascade's entries: its time keeps the trigger's levels that are > (X, c) and appends (X, c).
 // ---------------------------------------------------------------------------
 struct CvpProblem : LabelStore {
-  static constexpr bool CAN_SKIP = false;   // (the 8-lane CvpEllProblemT carries its own switch)
   static constexpr bool HAS_GOAL_TIME = true;
   EvTime goal_t;                            // pop time of the vertex that armed the goal cutoff (GroupCtl::goal_time); +inf: not armed
   static constexpr int STAGNATION = STAGNATION_ROUNDS;
@@ -212,21 +211,10 @@ struct CvpProblem : LabelStore {
 // lanes with shuffles.  Vertices with more than 8 faces take the CSR path on lane 0.
 // ---------------------------------------------------------------------------
 
-template <bool SKIP>
-struct CvpEllProblemT : CvpProblem {
+struct CvpEllProblem : CvpProblem {
   static constexpr bool TWO_SOURCES = true;   // an ELL slot names the two source vertices of a face
-  // Clean-candidate skip (band_engine.cuh): a candidate's label is a pure function of its sources' labels (+ the band end
-  // through `d < band_end`); it is re-evaluated only if a source was re-labelled in or after the round of its last
-  // evaluation.  Both stamps are 1-based round numbers and only ever compared across a group barrier.
-  static constexpr bool CAN_SKIP = SKIP;      // compile-time: the default instantiation carries none of the bookkeeping
   // whole-grid main pass: plain causal candidates one per thread (eval_plain), the rest on 8 lanes (run_band_rounds_sub8)
-  static constexpr bool PLAIN_FAST = !SKIP;
-  uint32_t* last_eval;     // round + 1 of the last evaluation; 0 = never evaluated
-  uint32_t* dirty_round;   // round + 1 of the last re-label of a face neighbour; 0 = never
-  uint32_t* excl_min;      // float bits: smallest finite source label that lay beyond the band end at the last evaluation and
-                           // could still fire before the candidate pops (d <= its pop time); +inf: none.  The candidate is
-                           // re-evaluated once the band end passes it.
-  int skip_clean;          // runtime switch (0: every candidate is recomputed every round)
+  static constexpr bool PLAIN_FAST = true;
   // activation marks of the two source vertices: fetched together with their labels (whole-grid single plan: one L2 trip
   // less on the evaluation that activates, which is on the wave's critical path) or only by that one evaluation
   // (throughput-bound batches: two scattered 4-byte loads = 64 L1 wavefronts per warp less on every other evaluation)
@@ -363,14 +351,13 @@ struct CvpEllProblemT : CvpProblem {
   // activation marks of the lane's two source vertices (fetched together with their labels).
   __device__ __forceinline__ void replay_sub8(uint32_t c, uint32_t j, bool has, const int4& ix, const float4& w, float band_end,
                                               float goal, uint32_t round, const uint32_t* mark, const EvTime& old_t, float& nd, EvTime& nt, int& deg_out,
-                                              uint32_t& mk1, uint32_t& mk2, float& excl_min_out) const {
+                                              uint32_t& mk1, uint32_t& mk2) const {
     constexpr unsigned FULL = 0xffffffffu;
     const float INF = __uint_as_float(INF_BITS);
     const int deg = __shfl_sync(FULL, ix.w, 0, 8);
     deg_out = deg;
     bool big = has && deg > (int)ELL_W;     // (also set below when the replay meets a cascade deeper than 3 levels)
     bool valid = has && !big && ix.x != ELL_EMPTY;
-    float excl = INF;                                   // smallest finite source label of this lane's face beyond the band end
     EvTime T = ev_normal(INF, 0x7fffffffu);
     uint32_t Tv = 0x7fffffffu;
     double U = 0.0, X = 0.0;
@@ -384,10 +371,6 @@ struct CvpEllProblemT : CvpProblem {
       const double2 g01 = __ldg(gp), g23 = __ldg(gp + 1);
       FaceGeo g; g.p = g01.x; g.hc = g01.y; g.t0a = g23.x;
       const Label a = unpack_label(v1, sa), b = unpack_label(v2, sb);
-      if constexpr (SKIP) {
-        if (__float_as_uint(a.d) != INF_BITS && !(a.d < band_end)) excl = a.d;
-        if (__float_as_uint(b.d) != INF_BITS && !(b.d < band_end)) excl = fminf(excl, b.d);
-      }
       valid = face_time(c, v1, v2, a, b, band_end, goal, T, Tv);
       if (valid) {
         eval_face_geo((double)a.d, (double)b.d, (double)w.z, (double)w.y, (double)w.x, g, U, X);
@@ -495,15 +478,6 @@ struct CvpEllProblemT : CvpProblem {
         cur = cs; tc = ts;
       }
     }
-    if constexpr (!SKIP) excl_min_out = 0.0f;
-    else {
-      // a source beyond the band end matters only if its face could fire before c pops: the face time's first level is
-      // >= the source's label, so labels above c's pop time are irrelevant until c itself is re-labelled
-      float e = (excl <= tc.a1) ? excl : INF;
-#pragma unroll
-      for (int o = 4; o > 0; o >>= 1) e = fminf(e, __shfl_xor_sync(FULL, e, o, 8));
-      excl_min_out = big ? 0.0f : e;                    // CSR path: not tracked per source, re-evaluated every round
-    }
     const unsigned anybig = __ballot_sync(FULL, big);
     if (anybig) {
       cur = __shfl_sync(FULL, cur, 0, 8);
@@ -513,9 +487,6 @@ struct CvpEllProblemT : CvpProblem {
     nd = cur; nt = tc;
   }
 };
-
-using CvpEllProblem = CvpEllProblemT<false>;
-using CvpEllSkipProblem = CvpEllProblemT<true>;
 
 // ---------------------------------------------------------------------------
 // Inflation: multi-source FMM from the lethal set (InflationLayer::waveCostInflation,
@@ -691,7 +662,7 @@ struct InflationProblem : LabelStore {
     nd = cur; tc_out = tc;
   }
 
-  // Same collapse as CvpEllProblemT::replay_sub8's fast path: if every firing face either is causal (candidate above its own
+  // Same collapse as CvpEllProblem::replay_sub8's fast path: if every firing face either is causal (candidate above its own
   // pop time) with both sources inside the radius (so the accepted value is also the heap key, :310), or fires after the
   // smallest causal candidate m, the call-ordered replay yields d = m and the pop time (m, c) -- no sorting of the faces,
   // no visit keys.  Returns false if the general replay is needed.
@@ -816,9 +787,7 @@ using DijkstraProblem = DijkstraProblemT<uint4>;
 // ---------------------------------------------------------------------------
 struct DijkstraEllProblem : DijkstraProblem {
   static constexpr bool TWO_SOURCES = false;
-  static constexpr bool CAN_SKIP = false;     // one relaxation is as cheap as the bookkeeping of skipping it
   static constexpr bool PLAIN_FAST = false;
-  uint32_t* last_eval = nullptr; uint32_t* dirty_round = nullptr; uint32_t* excl_min = nullptr; int skip_clean = 0;
   static constexpr bool prefetch_marks = true;
   const uint4* __restrict__ ell_adj;
   uint32_t* ver;
@@ -856,8 +825,7 @@ struct DijkstraEllProblem : DijkstraProblem {
   }
   __device__ __forceinline__ void replay_sub8(uint32_t c, uint32_t j, bool has, const int4& ix, const float4&, float band_end,
                                               float goal, uint32_t /*round*/, const uint32_t* mark, const EvTime& /*old_t*/, float& nd, EvTime& nt, int& deg_out,
-                                              uint32_t& mk1, uint32_t& mk2, float& excl_min_out) const {
-    excl_min_out = 0.0f;
+                                              uint32_t& mk1, uint32_t& mk2) const {
     constexpr unsigned FULL = 0xffffffffu;
     const float INF = __uint_as_float(INF_BITS);
     const int deg = __shfl_sync(FULL, ix.w, 0, 8);

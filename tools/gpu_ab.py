@@ -1,7 +1,8 @@
 """Dev script (GPU box): A/B of the opt-in variants written without GPU access (round 1), one call, ~2 GPU-minutes.
   python tools/gpu_ab.py [grid side of the single-plan mesh, default 2240]
 Prints, for each variant, kernel time + the bit-equality against the default kernel:
-  * clean-candidate skip: whole-grid single CVP plan (5 M) and the per-CTA batch (1 M, 2 goals per SM = one wave)
+  * in-round sweeps / band width of the whole-grid single CVP plan (5 M), band width of the per-CTA batch (1 M, 2 goals
+    per SM = one wave)
   * k_layers<true> (shared-memory seen-set) on the 5 M mesh
   * the dynamic-obstacle cycle (inflation update, vector field, incremental layerChanged vs full re-install)"""
 import ctypes as C, sys, time
@@ -14,21 +15,11 @@ from mesh_navigation_b200.api import MeshMap, CVPMeshPlanner, InflationLayer
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 2240
 pos, faces = synth.grid_mesh(n, n, terrain=True)
 mm = MeshMap(pos, faces); ed = mm.edgeDistances(); vc = np.zeros(mm.V, np.float32); mm.setCosts(vc, ed)
-for f in ("mnb_debug_set_skip_clean", "mnb_debug_set_layers_smem"):
-    getattr(mm.L, f).argtypes = [C.c_void_p, C.c_int32]
+mm.L.mnb_debug_set_layers_smem.argtypes = [C.c_void_p, C.c_int32]
 c = synth.nearest_vertex(pos, [n * 0.05, n * 0.05, float(pos[:, 2].mean())])
 sf = int(2 * ((c // n) * (n - 1) + (c % n))); sp = pos[faces[sf]].mean(0).astype(np.float32)
 pl = CVPMeshPlanner(mm)
-ref = None
-for skip in (0, 1, 0, 1):
-    mm.L.mnb_debug_set_skip_clean(mm._ctx, skip)
-    best = 1e9
-    for it in range(3):
-        g = pl.waveFrontPropagation(sf, sp); best = min(best, g['kernel_ms'])
-    if ref is None: ref = g['dist'].copy()
-    print(f"[single {n}x{n}] skip_clean={skip}: kernel {best:.2f} ms rounds {g['rounds']} recomputes/V {g['recomputes']/mm.V:.2f} "
-          f"skipped/V {g['skipped']/mm.V:.2f} dist!=default {int((g['dist'].view(np.uint32) != ref.view(np.uint32)).sum())}", flush=True)
-mm.L.mnb_debug_set_skip_clean(mm._ctx, 0)
+ref = pl.waveFrontPropagation(sf, sp)['dist'].copy()
 # band width / in-round sweeps were tuned (1.8 m / 15) before the causal collapse made an evaluation cheaper: re-scan
 mm.L.mnb_debug_set_sweeps.argtypes = [C.c_void_p, C.c_int32]
 for (k, delta) in ((15, 1.8), (10, 1.2), (20, 2.4), (30, 3.6), (24, 1.8), (8, 1.8), (0, 0.3)):
@@ -70,25 +61,11 @@ mm.close()
 nb = 1000
 bpos, bfaces = synth.grid_mesh(nb, nb, terrain=True)
 bm = MeshMap(bpos, bfaces); bm.setCosts(np.zeros(bm.V, np.float32), bm.edgeDistances())
-bm.L.mnb_debug_set_skip_clean.argtypes = [C.c_void_p, C.c_int32]
 G = 2 * torch.cuda.get_device_properties(0).multi_processor_count     # one wave: 2 CTAs per SM
 goals = synth.batch_goal_vertices(bm.V, G, seed=1234)
 gi, gj = np.minimum(goals % nb, nb - 2), np.minimum(goals // nb, nb - 2)
 sfs = (2 * (gj * (nb - 1) + gi)).astype(np.uint32); sps = bpos[bfaces[sfs]].mean(1).astype(np.float32)
 out = torch.empty((G, bm.V), dtype=torch.float32, device='cuda')
-bref = None
-for skip in (0, 1, 0, 1):
-    bm.L.mnb_debug_set_skip_clean(bm._ctx, skip)
-    bm.use_device_pointers(True)
-    for rep in range(2):
-        t = time.perf_counter(); bm.cvp_batch_dev(sfs, sps, 1.0, out.data_ptr()); torch.cuda.synchronize(); dt = time.perf_counter() - t
-    bm.use_device_pointers(False)
-    st = bm.stats()
-    cur = out[:8].cpu().numpy()
-    if bref is None: bref = cur.copy()
-    print(f"[batch {G} x 1M] skip_clean={skip}: {1e3*dt:.1f} ms -> {G/dt:.1f} plans/s, kernel {st['kernel_ms']:.1f} ms, recomputes/V {st['recomputes']/G/bm.V:.2f} "
-          f"skipped/V {st['skipped']/G/bm.V:.2f} first 8 fields != default: {int((cur.view(np.uint32) != bref.view(np.uint32)).sum())}", flush=True)
-bm.L.mnb_debug_set_skip_clean(bm._ctx, 0)
 for delta in (0.2, 0.3, 0.45, 0.6):
     bm.set_tuning(delta, 1, 0)
     bm.use_device_pointers(True)

@@ -1,13 +1,12 @@
 """Dev script (GPU box): A/B of batch-kernel builds / cluster sizes / band widths on the config-4 mesh.
-  python tools/gpu_batch2.py <grid side> <spec> [<spec> ...]      spec = lib:cluster:goals:delta[:legacy]
+  python tools/gpu_batch2.py <grid side> <spec> [<spec> ...]      spec = lib:cluster:goals:delta
 lib = path of a libmeshnav_b200.so build ('-' = the in-tree one); one subprocess per spec (a process loads one build).
 Every spec prints plans/s, kernel ms, rounds and recomputes per plan, and a checksum of the potentials (all builds must agree)."""
 import os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-def worker(n, lib, cs, ng, delta, legacy):
+def worker(n, lib, cs, ng, delta):
     sys.path.insert(0, ROOT)
-    if legacy: os.environ["MNB_BATCH_LEGACY"] = "1"
     from mesh_navigation_b200 import _lib
     if lib != "-": _lib.LIB_PATH = os.path.join(ROOT, lib)
     import time, zlib, numpy as np, torch
@@ -27,15 +26,15 @@ def worker(n, lib, cs, ng, delta, legacy):
     mm.use_device_pointers(False)
     st = mm.stats()
     chk = zlib.crc32(out[: min(ng, 8)].cpu().numpy().tobytes())
-    print(f"n={n} lib={lib} legacy={int(legacy)} cluster={cs} goals={ng} delta={delta}: {best*1e3:.1f} ms -> {ng/best:.1f} plans/s, kernel {st['kernel_ms']:.1f} ms "
+    print(f"n={n} lib={lib} cluster={cs} goals={ng} delta={delta}: {best*1e3:.1f} ms -> {ng/best:.1f} plans/s, kernel {st['kernel_ms']:.1f} ms "
           f"rounds/plan {st['rounds']/ng:.0f} recomp/V {st['recomputes']/ng/mm.V:.2f} crc {chk:08x}", flush=True)
 
 if __name__ == "__main__":
     if sys.argv[1] == "--worker":
-        worker(int(sys.argv[2]), sys.argv[3], int(sys.argv[4]), int(sys.argv[5]), float(sys.argv[6]), sys.argv[7] == "1")
+        worker(int(sys.argv[2]), sys.argv[3], int(sys.argv[4]), int(sys.argv[5]), float(sys.argv[6]))
     else:
         n = sys.argv[1]
         for spec in sys.argv[2:]:
             f = spec.split(":")
-            r = subprocess.run([sys.executable, __file__, "--worker", n, f[0], f[1], f[2], f[3], "1" if len(f) > 4 else "0"], capture_output=True, text=True, timeout=600)
+            r = subprocess.run([sys.executable, __file__, "--worker", n, f[0], f[1], f[2], f[3]], capture_output=True, text=True, timeout=600)
             print((r.stdout.strip() or ("FAILED: " + r.stderr[-400:])), flush=True)

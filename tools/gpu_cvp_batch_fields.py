@@ -114,7 +114,7 @@ def main():
     used1 = used_bytes(torch)
     fields_call(mm, sfs, sps, bufs)
     ws_bytes = used_bytes(torch) - used1          # the workspace stays allocated after the call
-    ws_per_wave = 68 * V + 4 * max(65536, 2 * V)  # ensure_workspace: 76 bytes per vertex on large maps (+ a GroupCtl)
+    ws_per_wave = 56 * V + 4 * max(65536, 2 * V)  # ensure_workspace: 64 bytes per vertex on large maps (+ a GroupCtl)
     for _ in range(args.warmup):
         dist_call(mm, sfs, sps, bufs); fields_call(mm, sfs, sps, bufs)
     t_f, t_d, k_f, k_d, st_f, st_d = [], [], [], [], None, None
@@ -174,7 +174,7 @@ def main():
         st = fields_call(mm, sfs, sps, bufs)
         t1 = time.perf_counter() - t0
         ws = used_bytes(torch) - used0
-        ws_per_wave = 68 * V + 4 * max(65536, 2 * V)
+        ws_per_wave = 56 * V + 4 * max(65536, 2 * V)
         leg = {"mesh_vertices": int(V), "goals": int(n), "outputs": "dist + pred + direction + cutting face, device pointers",
                "ballast_bytes": ballast_bytes, "free_bytes_before_call": int(total - used0),
                "workspace_bytes_from_device_memory_growth": int(ws), "wavefronts_in_flight_from_workspace": int(ws // ws_per_wave),
