@@ -896,6 +896,8 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
 #ifdef MNB_GRID_TIMING
     if (gtid == 0) { ctl->t_ph[0] += (unsigned long long)(tps - tp0); ctl->t_ph[2] += cnt; }
 #endif
+    // sweep 0 appends to dn[0]: after an odd sweep count the previous round's last sweep left its count there
+    if constexpr (SW) if (threadIdx.x == 0) ss->dn[0] = 0;
     if constexpr (SW) for (int sw = 0; sw < n_sweeps; ++sw) {
 #ifdef MNB_GRID_TIMING
       const long long tq0 = clock64();

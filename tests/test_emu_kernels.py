@@ -27,12 +27,18 @@ GROUPS = [
     ("test_gpu_group.py", "sharded_batch"),
     ("test_gpu_raycast.py", "cast_rays or obstacle_layer or obstacle_update or normal_clearance"),
     ("test_gpu_updates.py", "layer_changed or max_combination or on_input_changed or vector_field or repulsive or clean_candidate or shared_memory_variant or high_degree or edge_cases or goal_cutoff_armed or deeply_nested or backstep_deep or seed_pops_after or never_fixed or batch_engine or abi_argument"),
+    ("test_gpu_launch_configs.py", "cvp_grid_threads"),
+    ("test_gpu_launch_configs.py", "cvp_cluster_kernels"),
+    ("test_gpu_launch_configs.py", "dijkstra_grid or dijkstra_cluster or inflation_threads"),
+    ("test_gpu_launch_configs.py", "capacity"),
 ]
 # the same tests under a randomised warp schedule (MNB_EMU_SHUFFLE, see tests/emu/cuda_runtime.h): warps are visited in a
 # different order on every scheduler pass and preempted at collectives, which turns a missing barrier into a failure
 SHUFFLED = [
     ("test_gpu_updates.py", "layer_changed or on_input_changed or vector_field or clean_candidate", "1"),
     (PARITY, "cvp_full_field or dijkstra_bit_exact or inflation_wave or backtrack or locate", "2"),
+    # block sizes below 512 and odd sweep counts on the whole-grid kernel
+    ("test_gpu_launch_configs.py", "cvp_grid_threads and (deep_cascade_planar or delaunay_hub)", "3"),
 ]
 
 
