@@ -143,6 +143,27 @@ int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_face
                              float* out_dist /* [n][V] or NULL */, uint32_t* out_pred /* [n][V] or NULL */,
                              float* out_direction /* [n][V] or NULL */, int32_t* out_cutting_face /* [n][V] or NULL */);
 
+/* Cost matrices: the cost from each of n seeds to each of m target vertices, e.g. from every candidate goal to every
+ * robot of a fleet, without the [n][V] rows.  out[k][j] ([n][m] row-major) is bit-identical to
+ * dist[k][target_vertices[j]] of mnb_dijkstra_batch (mnb_dijkstra_matrix) or of mnb_cvp_batch (mnb_cvp_matrix) with
+ * the same seeds and cost_limit: +inf where the target is unreached.  A wave stops as soon as every target has
+ * settled -- its label is then final -- so targets near their seeds cost a fraction of the full field; mnb_get_stats
+ * reports the settled vertices and rounds summed over the waves.  Duplicate seeds and duplicate targets are allowed.
+ * The seed and target arrays are always host pointers; out follows mnb_set_pointer_mode.  Errors, with nothing
+ * written: MNB_E_ARG for n == 0, m == 0 or a NULL array; MNB_E_STATE without costs; MNB_INVALID_START for a seed
+ * >= V (Dijkstra) or a seed face >= F (CVP); MNB_INVALID_GOAL for a target >= V.  MNB_CANCELED after mnb_cancel: no
+ * new goal is taken once the flag is set (the matrix is then incomplete).  No [n][V] rows are allocated in either
+ * pointer mode; the number of concurrent waves is capped as for the batch calls, by the workspace alone.
+ * mnb_dijkstra_matrix runs in mnb_dijkstra_batch's workspace: the results of the last mnb_cvp and of the last
+ * inflation stay available.  mnb_cvp_matrix shares the wavefront workspace like mnb_cvp_batch: the last inflation's
+ * labels are dropped, the outputs of the last mnb_cvp remain available. */
+int32_t mnb_dijkstra_matrix(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices /* n, host */,
+                            uint32_t m, const uint32_t* target_vertices /* m, host */, double cost_limit,
+                            float* out /* [n][m] */);
+int32_t mnb_cvp_matrix(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n, host */, const float* seed_pos /* 3n, host */,
+                       uint32_t m, const uint32_t* target_vertices /* m, host */, double cost_limit,
+                       float* out /* [n][m] */);
+
 /* ---- InflationLayer::waveCostInflation (inflation_layer.cpp:341-491) -----
  * lethals[n] (any order, duplicates allowed).  Uses edge_distances (:383), not edge_weights.
  * out_dist[V]: distances_ (+inf = not in the sparse map); out_cost[V]: riskiness_ =

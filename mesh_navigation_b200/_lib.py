@@ -51,7 +51,8 @@ class Stats(C.Structure):
 EXPORTS = [
     "mnb_create", "mnb_destroy", "mnb_last_error", "mnb_set_pointer_mode", "mnb_stream", "mnb_set_mesh",
     "mnb_num_vertices", "mnb_num_faces", "mnb_num_edges", "mnb_get_edges", "mnb_get_edge_distances",
-    "mnb_compute_edge_weights", "mnb_set_costs", "mnb_dijkstra", "mnb_dijkstra_batch", "mnb_cvp", "mnb_cvp_batch", "mnb_cvp_batch_fields", "mnb_inflate",
+    "mnb_compute_edge_weights", "mnb_set_costs", "mnb_dijkstra", "mnb_dijkstra_batch", "mnb_cvp", "mnb_cvp_batch", "mnb_cvp_batch_fields",
+    "mnb_dijkstra_matrix", "mnb_cvp_matrix", "mnb_inflate",
     "mnb_cancel", "mnb_get_stats", "mnb_set_tuning", "mnb_compute_layers", "mnb_get_vertex_normals", "mnb_vector_map", "mnb_cvp_backtrack", "mnb_locate",
     "mnb_update_vertex_costs", "mnb_get_costs", "mnb_max_combination_update", "mnb_avg_combination_update", "mnb_inflation_update",
     "mnb_inflation_vector_map", "mnb_inflation_vector_at", "mnb_set_repulsive_field",
@@ -89,6 +90,8 @@ def load():
     L.mnb_cvp.restype = i32; L.mnb_cvp.argtypes = [vp, u32, vp, i64, dbl, dbl, vp, vp, vp, vp]
     L.mnb_cvp_batch.restype = i32; L.mnb_cvp_batch.argtypes = [vp, u32, vp, vp, dbl, vp]
     L.mnb_cvp_batch_fields.restype = i32; L.mnb_cvp_batch_fields.argtypes = [vp, u32, vp, vp, dbl, vp, vp, vp, vp]
+    L.mnb_dijkstra_matrix.restype = i32; L.mnb_dijkstra_matrix.argtypes = [vp, u32, vp, u32, vp, dbl, vp]
+    L.mnb_cvp_matrix.restype = i32; L.mnb_cvp_matrix.argtypes = [vp, u32, vp, vp, u32, vp, dbl, vp]
     L.mnb_inflate.restype = i32; L.mnb_inflate.argtypes = [vp, vp, u32, vp, C.POINTER(InflationParams), vp, vp]
     L.mnb_compute_layers.restype = i32; L.mnb_compute_layers.argtypes = [vp, C.POINTER(LayerParams), vp, vp, vp, vp]
     L.mnb_get_vertex_normals.restype = i32; L.mnb_get_vertex_normals.argtypes = [vp, vp]

@@ -248,6 +248,19 @@ class MeshMap:
         return self._check(self.L.mnb_cvp_batch_fields(self._ctx, sf.size, _p(sf), _p(sp), float(cost_limit), opt(d_dist),
                                                        opt(d_pred), opt(d_dir), opt(d_cut)))
 
+    def dijkstra_matrix_dev(self, seed_vertices, target_vertices, cost_limit, d_out: int) -> int:
+        """mnb_dijkstra_matrix with a device output ([n,m]); seeds and targets are host values"""
+        sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32).reshape(-1)
+        tv = np.ascontiguousarray(target_vertices, dtype=np.uint32).reshape(-1)
+        return self._check(self.L.mnb_dijkstra_matrix(self._ctx, sv.size, _p(sv), tv.size, _p(tv), float(cost_limit), _p(d_out)))
+
+    def cvp_matrix_dev(self, seed_faces, seed_pos, target_vertices, cost_limit, d_out: int) -> int:
+        """mnb_cvp_matrix with a device output ([n,m]); seeds and targets are host values"""
+        sf = np.ascontiguousarray(seed_faces, dtype=np.uint32).reshape(-1)
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
+        tv = np.ascontiguousarray(target_vertices, dtype=np.uint32).reshape(-1)
+        return self._check(self.L.mnb_cvp_matrix(self._ctx, sf.size, _p(sf), _p(sp), tv.size, _p(tv), float(cost_limit), _p(d_out)))
+
 
 class DijkstraMeshPlanner:
     """dijkstra_mesh_planner::DijkstraMeshPlanner -- wavefront part (dijkstra():217-398)."""
@@ -274,6 +287,16 @@ class DijkstraMeshPlanner:
         pred = np.empty((sv.size, m.V), dtype=np.uint32) if want_pred else None
         rc = m._check(m.L.mnb_dijkstra_batch(m._ctx, sv.size, _p(sv), float(self.cost_limit), _p(dist), _p(pred)))
         return dict(outcome=rc, dist=dist, pred=pred, **m.stats())
+
+    def costMatrix(self, seed_vertices, target_vertices):
+        """cost[k, j] = dijkstraBatch(seed_vertices)["dist"][k, target_vertices[j]], without the [n,V] rows: each wave
+        stops once its targets have settled"""
+        m = self.map
+        sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32).reshape(-1)
+        tv = np.ascontiguousarray(target_vertices, dtype=np.uint32).reshape(-1)
+        cost = np.empty((sv.size, tv.size), dtype=np.float32)
+        rc = m._check(m.L.mnb_dijkstra_matrix(m._ctx, sv.size, _p(sv), tv.size, _p(tv), float(self.cost_limit), _p(cost)))
+        return dict(outcome=rc, cost=cost, **m.stats())
 
     def computeVectorMap(self, pred):
         return self.map.vectorMap(pred)
@@ -353,6 +376,17 @@ class CVPMeshPlanner:
         rc = m._check(m.L.mnb_cvp_batch_fields(m._ctx, sf.size, _p(sf), _p(sp), float(self.cost_limit), _p(out["dist"]),
                                                _p(out["pred"]), _p(out["direction"]), _p(out["cutting_face"])))
         return dict(outcome=rc, **out, **m.stats())
+
+    def costMatrix(self, seed_faces, seed_pos, target_vertices):
+        """cost[k, j] = waveFrontPropagationBatch(seed_faces, seed_pos)["dist"][k, target_vertices[j]], without the
+        [n,V] rows: each wave stops once its targets have settled"""
+        m = self.map
+        sf = np.ascontiguousarray(seed_faces, dtype=np.uint32).reshape(-1)
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
+        tv = np.ascontiguousarray(target_vertices, dtype=np.uint32).reshape(-1)
+        cost = np.empty((sf.size, tv.size), dtype=np.float32)
+        rc = m._check(m.L.mnb_cvp_matrix(m._ctx, sf.size, _p(sf), _p(sp), tv.size, _p(tv), float(self.cost_limit), _p(cost)))
+        return dict(outcome=rc, cost=cost, **m.stats())
 
 
 class InflationLayer:

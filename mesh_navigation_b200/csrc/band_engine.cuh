@@ -311,7 +311,28 @@ struct GroupCtl {               // one per wavefront group, global memory
   unsigned long long t_work, t_flush, t_sync;   // clock cycles of thread 0 of the group: candidate loop / stage flush / barrier
   unsigned int barrier[2];      // grid_barrier state (whole-grid groups only)
   unsigned long long t_ph[8];   // phase cycles of thread 0 inside one candidate iteration (debug)
+  // matrix form of the batch kernels (TargetSet): distinct targets of the wave that have not settled yet, and the flag
+  // that ends the wave once none is left.  The flag is read at the top of a round like stop_ring, so it follows the same
+  // discipline: round r reads slot r&1, the thread that settles the last target in round r raises slot (r+1)&1.
+  int targets_left;
+  unsigned int done_ring[2];
 };
+
+// The matrix form of the batch kernels (mnb_dijkstra_matrix / mnb_cvp_matrix): a wave ends once every target vertex has
+// settled and writes only the labels of the targets.
+struct TargetSet {
+  const uint32_t* list;         // [m] device, the caller's order (duplicates allowed)
+  const uint32_t* bits;         // [V/32 + 1] device: bitmap of the distinct targets
+  uint32_t m, distinct;         // list length, number of distinct targets
+  float* out;                   // [n_queries][m]
+};
+
+// a list entry c settles in round r: if it is a target, count it; the thread that settles the last one raises the flag
+// the whole group reads at the top of round r + 1
+__device__ __forceinline__ void settle_target(GroupCtl* ctl, const uint32_t* bits, uint32_t c, uint32_t r) {
+  if ((__ldg(&bits[c >> 5]) >> (c & 31)) & 1u)
+    if (atomicSub(&ctl->targets_left, 1) == 1) atomicOr(&ctl->done_ring[(r + 1) & 1], 1u);
+}
 
 template <int CS>
 __device__ __forceinline__ void group_sync(unsigned int* bar = nullptr) {
@@ -400,13 +421,17 @@ __device__ __forceinline__ void stage_flush(S& st, uint32_t* list_next, unsigned
 //         (writes state/aux itself)
 //   void  activate(c, push)   calls push(x) for every vertex x that shares a face/edge with c
 //   bool  eligible(x)         may x ever receive a label
+//
+// TARGETS (matrix form): target_bits marks the target vertices, ctl->targets_left counts those that can still settle;
+// the loop ends once it reaches zero (settle_target).
 // -----------------------------------------------------------------------------
-template <int CS, class P>
+template <int CS, bool TARGETS = false, class P>
 __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_t* list1, uint32_t* mark,
                                 Stage& st, const float delta, const uint32_t gthreads, const uint32_t gtid,
                                 const int has_robot, const uint32_t r0, const uint32_t r1, const uint32_t r2,
                                 const double goal_dist_offset, const volatile int* cancel_flag,
-                                const float band_end_init, const uint32_t max_rounds) {
+                                const float band_end_init, const uint32_t max_rounds, const uint32_t* target_bits = nullptr) {
+  static_assert(!TARGETS || !P::CAN_SKIP, "targets are counted in the one-pass candidate loop only");
   float band_end_prev = band_end_init;  // > every seed potential: seeds are available from round 0
   unsigned long long my_recomputes = 0, my_settled = 0, my_skipped = 0;
   float lo_best = -1.0f; int stagnant = 0;       // best (largest) earliest-unsettled pop time seen so far
@@ -426,6 +451,9 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
     }
     const unsigned int stop = __ldcg(&ctl->stop_ring[r & 1]);
     if (n == 0 || stop || r > max_rounds) break;   // r is group-uniform: the watchdog cannot deadlock the barrier
+    // every target has settled.  The flag needs no carrying or clearing: the loop ends at the first round that reads it
+    // raised, so slot (r+1)&1 was read clear in round r-1 and nobody has written it since.
+    if constexpr (TARGETS) if (__ldcg(&ctl->done_ring[r & 1])) break;
     if (r > 0 && __float_as_uint(m_prev) == INF_BITS &&
         (__float_as_uint(lo_prev) == INF_BITS || lo_prev > goal)) break;
     // stagnation watch (all values are group-uniform): labels keep changing but the earliest unsettled pop
@@ -534,6 +562,7 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
         // converged prefix: the sequential algorithm has popped c with exactly this label
         mark[c] = MARK_FIXED;
         my_settled++;
+        if constexpr (TARGETS) settle_target(ctl, target_bits, c, r);
         if (has_robot && (c == r0 || c == r1 || c == r2)) {
           if (atomicSub(&ctl->robot_left, 1) == 1) {
             // c is not necessarily the last of the three in event order: take the latest pop time

@@ -265,7 +265,8 @@ __device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup
 //     across the round barrier; (2) is one float per vertex written by its own last evaluation.  On the terrain 64 % of
 //     the evaluations of the plain round loop find nothing changed; this phase costs them ~25 thread-instructions.
 //   B (8 lanes per candidate): the evaluation proper, on the compacted work queue.
-template <int CS, class Args>
+// TARGETS (matrix form): the loop ends once every target of a.tg has settled, as in run_band_rounds.
+template <int CS, bool TARGETS = false, class Args>
 __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const BatchGroup& G, uint32_t* list0, uint32_t* list1, BatchStage& st,
                                                       BatchWork& wk, const float delta, const uint32_t gthreads, const uint32_t gtid,
                                                       const BatchSeeds& sd, const float band_end_init) {
@@ -287,6 +288,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
     const float lo_prev = __uint_as_float(__ldcg(&ctl->lo[prev]));
     const unsigned int stop = __ldcg(&ctl->stop_ring[r & 1]);
     if (n == 0 || stop || r > a.max_rounds) break;           // r is group-uniform: the watchdog cannot deadlock the barrier
+    if constexpr (TARGETS) if (__ldcg(&ctl->done_ring[r & 1])) break;     // every target has settled (see run_band_rounds)
     if (r > 0 && __float_as_uint(m_prev) == INF_BITS && __float_as_uint(lo_prev) == INF_BITS) break;
     // stagnation watch (see run_band_rounds): labels keep changing but the earliest unsettled pop time does not move
     if (r > 0 && __float_as_uint(m_prev) != INF_BITS && !(lo_prev > lo_best)) { if (++stagnant >= STAGNATION_ROUNDS) strict = 1; }
@@ -317,6 +319,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
           const uint32_t c = ce & ~LIST_ACTIVATED;
           tau = __uint_as_float(__ldcg(reinterpret_cast<const uint32_t*>(G.state) + 4 * (size_t)c + 1));
           settled = tau < m_prev && tau < band_end_prev;   // converged prefix: the sequential algorithm has popped c with this label
+          if constexpr (TARGETS) if (settled) settle_target(ctl, a.tg.bits, c, r);
           if (!settled) {
             const uint4 sk = __ldcg(&G.skipw[c]);
             const uint32_t dmb = buf_prev ? sk.y : sk.x;

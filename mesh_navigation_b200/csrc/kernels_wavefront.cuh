@@ -53,6 +53,12 @@ struct CvpKernelArgs {
   int sweeps;                   // in-round sweeps of a single plan (0 = off, -1 = from the band width)
   float hop;                    // ~ one dependency hop in potential units (1.35 x mean edge weight)
 };
+// the arguments of the matrix form of k_cvp_batch.  A type of its own rather than a field of CvpKernelArgs: the batch
+// kernels pass their arguments by reference to out-of-line functions, which copy them to the stack, so a larger
+// CvpKernelArgs would grow the stack frame of every CVP batch kernel.
+struct CvpMatrixArgs : CvpKernelArgs {
+  TargetSet tg;
+};
 
 template <int CS>
 __device__ __forceinline__ void group_coords(uint32_t& g, uint32_t& gthreads, uint32_t& gtid) {
@@ -71,6 +77,27 @@ __device__ __forceinline__ void ctl_reset(GroupCtl* ctl, unsigned int n0, float 
   ctl->goal_bits = INF_BITS; ctl->robot_left = 0;
   ctl->goal_time[0] = INF_BITS; ctl->goal_time[1] = 0u; ctl->goal_time[2] = 0u; ctl->goal_time[3] = 0u; ctl->goal_time[4] = 0u; ctl->goal_time[5] = 0u;
   ctl->pool_top = 0u;
+  ctl->done_ring[0] = 0u; ctl->done_ring[1] = 0u;
+}
+
+// Matrix form, after the seeding (and a group barrier): ctl->targets_left = tg.distinct less the targets that are done
+// before the first round -- a seed (MARK_FIXED: its label is final) or a vertex that never becomes a candidate
+// (eligible(v) false: its entry stays +inf).  If none is left the flag of round 0 is raised and the wave runs no round.
+// Called by every thread of the group; a group barrier must follow.
+template <class Eligible>
+__device__ __forceinline__ void count_targets_done_at_init(const TargetSet& tg, GroupCtl* ctl, const uint32_t* mark, uint32_t V,
+                                                           uint32_t gthreads, uint32_t gtid, Eligible eligible) {
+  unsigned int done = 0;
+  for (uint32_t w = gtid; w <= (V >> 5); w += gthreads) {
+    uint32_t b = __ldg(&tg.bits[w]);
+    while (b) {
+      const uint32_t v = (w << 5) + (uint32_t)(__ffs(b) - 1);
+      b &= b - 1u;
+      if (__ldcg(&mark[v]) == MARK_FIXED || !eligible(v)) done++;
+    }
+  }
+  done = __reduce_add_sync(0xffffffffu, done);
+  if ((threadIdx.x & 31) == 0 && done && atomicSub(&ctl->targets_left, (int)done) == (int)done) atomicOr(&ctl->done_ring[0], 1u);
 }
 
 #include "batch_engine.cuh"
@@ -240,8 +267,13 @@ __device__ __noinline__ void batch_fields_epilogue(const CvpKernelArgs& a, const
 
 // FIELDS = false: potentials only (mnb_cvp_batch, and mnb_cvp_batch_fields asked for potentials alone).  FIELDS = true:
 // each group also runs the epilogue of its goal before it takes the next one, and takes none once the cancel flag is set.
-template <int CS, bool FIELDS>
-__global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_batch(const CvpKernelArgs a) {
+// Args = CvpMatrixArgs (with FIELDS = false; mnb_cvp_matrix): the matrix form.  A wave ends once the target vertices of
+// a.tg have settled and writes their potentials, row q of a.tg.out, instead of the V-sized row; no new goal is taken once
+// the cancel flag is set.
+template <int CS, bool FIELDS, class Args = CvpKernelArgs>
+__global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_batch(const Args a) {
+  constexpr bool MATRIX = std::is_same_v<Args, CvpMatrixArgs>;
+  static_assert(!(FIELDS && MATRIX), "the matrix form writes potentials only");
   __shared__ BatchStage st;
   __shared__ BatchWork wk;
   uint32_t g, gthreads, gtid;
@@ -258,7 +290,7 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
   __syncthreads();
   for (;;) {
     if (gtid == 0) {
-      if constexpr (FIELDS) ctl->query = (a.cancel_flag && *(const volatile int*)a.cancel_flag) ? a.n_queries : atomicAdd(a.next_query, 1u);
+      if constexpr (FIELDS || MATRIX) ctl->query = (a.cancel_flag && *(const volatile int*)a.cancel_flag) ? a.n_queries : atomicAdd(a.next_query, 1u);
       else ctl->query = atomicAdd(a.next_query, 1u);
     }
     group_sync<CS>();
@@ -301,11 +333,21 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
         }
       }
       ctl_reset(ctl, n0, seed_min);
+      if constexpr (MATRIX) ctl->targets_left = (int)a.tg.distinct;
     }
     group_sync<CS>();
-    run_band_rounds_batch<CS>(a, G, list0, list1, st, wk, a.delta, gthreads, gtid, sd, nextafterf(sd.seed_max, __uint_as_float(INF_BITS)));
+    if constexpr (MATRIX) {
+      count_targets_done_at_init(a.tg, ctl, G.mark, V, gthreads, gtid, [&](uint32_t v) {   // candidates: k_cvp_batch's activation test
+        return !(a.invalid && a.invalid[v]) && !((double)a.cost[v] >= a.cost_limit);
+      });
+      group_sync<CS>();
+    }
+    run_band_rounds_batch<CS, MATRIX>(a, G, list0, list1, st, wk, a.delta, gthreads, gtid, sd, nextafterf(sd.seed_max, __uint_as_float(INF_BITS)));
     group_sync<CS>();
-    if (a.out_dist) {
+    if constexpr (MATRIX) {
+      float* om = a.tg.out + (size_t)q * a.tg.m;
+      for (uint32_t j = gtid; j < a.tg.m; j += gthreads) om[j] = __uint_as_float(__ldcg(&G.state[a.tg.list[j]]).x);
+    } else if (a.out_dist) {
       float* od = a.out_dist + (size_t)q * V;
       for (uint32_t v = gtid; v < V; v += gthreads) od[v] = __uint_as_float(__ldcg(&G.state[v]).x);
     }
@@ -494,9 +536,12 @@ struct DijkstraBatchArgs {
   unsigned int* next_query;
   const int* cancel_flag;
   uint32_t max_rounds;
+  TargetSet tg;                 // k_dijkstra_batch<CS, true> only
 };
 
-template <int CS>
+// MATRIX (mnb_dijkstra_matrix): a wave ends once the target vertices of a.tg have settled and writes their distances, row
+// q of a.tg.out, instead of the V-sized rows.
+template <int CS, bool MATRIX = false>
 __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijkstra_batch(const DijkstraBatchArgs a) {
   __shared__ Stage st;
   uint32_t g, gthreads, gtid;
@@ -534,12 +579,21 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijk
         if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
       });
       ctl_reset(ctl, n0, 0.0f);
+      if constexpr (MATRIX) ctl->targets_left = (int)a.tg.distinct;
     }
     group_sync<CS>();
-    run_band_rounds<CS>(prob, ctl, list0, list1, mark, st, a.delta, gthreads, gtid, 0, 0xffffffffu, 0xffffffffu, 0xffffffffu,
-                        0.0, a.cancel_flag, 1e-30f, a.max_rounds);
+    if constexpr (MATRIX) {
+      // over-cost vertices are eligible: they get labels and settle like any other
+      count_targets_done_at_init(a.tg, ctl, mark, V, gthreads, gtid, [&](uint32_t v) { return prob.eligible(v); });
+      group_sync<CS>();
+    }
+    run_band_rounds<CS, MATRIX>(prob, ctl, list0, list1, mark, st, a.delta, gthreads, gtid, 0, 0xffffffffu, 0xffffffffu, 0xffffffffu,
+                                0.0, a.cancel_flag, 1e-30f, a.max_rounds, a.tg.bits);
     group_sync<CS>();
-    if (a.out_dist) {
+    if constexpr (MATRIX) {
+      float* om = a.tg.out + (size_t)q * a.tg.m;
+      for (uint32_t j = gtid; j < a.tg.m; j += gthreads) om[j] = __ldcg(&label[a.tg.list[j]]);
+    } else if (a.out_dist) {
       float* od = a.out_dist + (size_t)q * V;
       for (uint32_t v = gtid; v < V; v += gthreads) od[v] = __ldcg(&label[v]);
     }

@@ -66,6 +66,8 @@ struct mnb_ctx {
   float* d_out_dist = nullptr; size_t out_dist_cap = 0;
   uint32_t* d_out_pred = nullptr; float* d_out_dir = nullptr; int32_t* d_out_cut = nullptr;
   uint32_t* d_seed_faces = nullptr; float* d_seed_pos = nullptr; uint32_t seed_cap = 0;
+  // target vertices of the cost-matrix calls: the caller's list and the bitmap of the distinct ones (V/32 + 1 words)
+  uint32_t* d_targets = nullptr; uint32_t targets_cap = 0; uint32_t* d_target_bits = nullptr;
   float* d_face_normals = nullptr; float* d_vertex_normals = nullptr; uint8_t* d_border = nullptr;
   float* d_layer_costs = nullptr; float* d_layer_combined = nullptr; uint8_t* d_layer_mask = nullptr; float* d_clearance = nullptr;
   float4* d_pos4 = nullptr; float4* d_vn4 = nullptr; uint32_t* d_nbr8 = nullptr;     // packed copies for k_layers<true>
@@ -137,6 +139,7 @@ static void free_mesh(mnb_ctx* c) {
   dfree(c->dws.label); dfree(c->dws.mark); dfree(c->dws.list0); dfree(c->dws.list1); dfree(c->dws.ctl); c->dws_groups = 0;
   dfree(c->d_batch_pred); c->batch_pred_cap = 0; dfree(c->d_batch_dir); c->batch_dir_cap = 0; dfree(c->d_batch_cut); c->batch_cut_cap = 0;
   dfree(c->d_out_dist); c->out_dist_cap = 0; dfree(c->d_out_pred); dfree(c->d_out_dir); dfree(c->d_out_cut);
+  dfree(c->d_targets); c->targets_cap = 0; dfree(c->d_target_bits);
   dfree(c->d_infl_invalid); dfree(c->d_out_cost);
   dfree(c->d_infl_vec); dfree(c->d_infl_dist); dfree(c->d_infl_src); dfree(c->d_infl_flag);
   c->infl_labels_valid = false; c->infl_field_valid = false; c->repulsive_on = false;
@@ -627,6 +630,39 @@ static int32_t ensure_seeds(mnb_ctx* ctx, uint32_t n) {
   return MNB_OK;
 }
 
+// The targets of a cost-matrix call (mnb_dijkstra_matrix, mnb_cvp_matrix): host list, [n][m] output in the pointer mode.
+struct MatrixRequest { uint32_t m; const uint32_t* targets; float* out; };
+
+// MNB_INVALID_GOAL if a target is >= V (nothing written)
+static int32_t check_targets(mnb_ctx* ctx, const MatrixRequest* mx) {
+  if (mx) for (uint32_t j = 0; j < mx->m; ++j) if (mx->targets[j] >= ctx->V) return MNB_INVALID_GOAL;
+  return MNB_OK;
+}
+
+// Uploads the target list and the bitmap of the distinct targets (ctx buffers, freed with the mesh) and fills tg but out.
+static int32_t upload_targets(mnb_ctx* ctx, const MatrixRequest& mx, TargetSet& tg) {
+  const size_t words = ((size_t)ctx->V >> 5) + 1;
+  if (!ctx->d_target_bits) CK(dalloc(&ctx->d_target_bits, words));
+  if (mx.m > ctx->targets_cap) { dfree(ctx->d_targets); ctx->targets_cap = 0; CK(dalloc(&ctx->d_targets, (size_t)mx.m)); ctx->targets_cap = mx.m; }
+  std::vector<uint32_t> bits(words, 0u);     // (a copy from pageable memory has read it when cudaMemcpyAsync returns)
+  uint32_t distinct = 0;
+  for (uint32_t j = 0; j < mx.m; ++j) {
+    const uint32_t v = mx.targets[j], bit = 1u << (v & 31);
+    if (!(bits[v >> 5] & bit)) { bits[v >> 5] |= bit; ++distinct; }
+  }
+  CK(cudaMemcpyAsync(ctx->d_target_bits, bits.data(), sizeof(uint32_t) * words, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->d_targets, mx.targets, sizeof(uint32_t) * mx.m, cudaMemcpyHostToDevice, ctx->stream));
+  tg.list = ctx->d_targets; tg.bits = ctx->d_target_bits; tg.m = mx.m; tg.distinct = distinct;
+  return MNB_OK;
+}
+
+// host-pointer mode: the [n][m] matrix from its device staging (d_out_dist) into the caller's array
+static int32_t copy_matrix_out(mnb_ctx* ctx, uint32_t n, const MatrixRequest* mx) {
+  if (mx && ctx->ptr_mode != MNB_PTR_DEVICE)
+    CK(cudaMemcpyAsync(mx->out, ctx->d_out_dist, sizeof(float) * n * (size_t)mx->m, cudaMemcpyDeviceToHost, ctx->stream));
+  return MNB_OK;
+}
+
 static void fill_cvp_args(mnb_ctx* ctx, CvpKernelArgs& a) {
   a.V = ctx->V; a.pos = ctx->d_pos; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx;
   a.cor_w = ctx->d_cor_w; a.ell_idx = ctx->d_ell_idx; a.ell_w = ctx->d_ell_w; a.ell_geo = ctx->d_ell_geo; a.cost = ctx->d_cost; a.invalid = ctx->has_invalid ? ctx->d_invalid : nullptr; a.ws = ctx->ws;
@@ -717,17 +753,21 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
 // (k_cvp_batch<CS, true>) each wavefront runs the epilogue of its goal before its group takes the next one; potentials
 // alone run the potentials-only kernel.  The waves share the wavefront workspace with single plans and inflation (not the
 // single plan's outputs), and their number is capped by the free device memory as well as by the CTA slots.
+// With mx (mnb_cvp_matrix; no row outputs) the waves run the matrix form k_cvp_batch<CS, false, CvpMatrixArgs> into mx->out.
 static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
-                                     float* out_dist, uint32_t* out_pred, float* out_dir, int32_t* out_cut) {
-  if (!ctx || !seed_faces || !seed_pos || (!out_dist && !out_pred && !out_dir && !out_cut) || !ctx->V || n == 0) return MNB_E_ARG;
+                                     float* out_dist, uint32_t* out_pred, float* out_dir, int32_t* out_cut,
+                                     const MatrixRequest* mx = nullptr) {
+  if (!ctx || !seed_faces || !seed_pos || (!out_dist && !out_pred && !out_dir && !out_cut && !mx) || !ctx->V || n == 0) return MNB_E_ARG;
   if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
   for (uint32_t i = 0; i < n; ++i) if (seed_faces[i] >= ctx->F) return MNB_INVALID_START;
-  CK(cudaSetDevice(ctx->device));
   int32_t rc;
+  if ((rc = check_targets(ctx, mx)) != MNB_OK) return rc;
+  CK(cudaSetDevice(ctx->device));
   const size_t V = ctx->V, rows = (size_t)n * V;
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   const bool fields = out_pred || out_dir || out_cut;
   if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
+  if (mx && !dev && (rc = ensure_out(ctx, (size_t)n * mx->m, false)) != MNB_OK) return rc;
   if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized; the
                        // single plan's outputs stay untouched for mnb_cvp_backtrack / mnb_vector_map)
     if (out_dist && (rc = ensure_out(ctx, rows, false)) != MNB_OK) return rc;
@@ -745,7 +785,8 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
     }
   }
   int cs = 1; unsigned groups = 1;
-  rc = fields ? batch_shape(ctx, k_cvp_batch<1, true>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
+  rc = mx ? batch_shape(ctx, k_cvp_batch<1, false, CvpMatrixArgs>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
+     : fields ? batch_shape(ctx, k_cvp_batch<1, true>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
               : batch_shape(ctx, k_cvp_batch<1, false>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups);
   if (rc != MNB_OK) return rc;
   if ((rc = ensure_workspace(ctx, groups)) != MNB_OK) return rc;
@@ -755,22 +796,29 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
   CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
-  CvpKernelArgs a{};
+  CvpMatrixArgs a{};
   fill_cvp_args(ctx, a);
   a.n_queries = n; a.robot_face = -1; a.cost_limit = cost_limit; a.goal_dist_offset = 0.0;
   a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
   a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
   a.out_dir = !out_dir ? nullptr : (dev ? out_dir : ctx->d_batch_dir);
   a.out_cut = !out_cut ? nullptr : (dev ? out_cut : ctx->d_batch_cut);
+  if (mx) {
+    if ((rc = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return rc;
+    a.tg.out = dev ? mx->out : ctx->d_out_dist;
+  }
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   const unsigned blocks = groups * (unsigned)cs;
   const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
     constexpr int CS = decltype(c)::value;
-    return fields ? launch_cluster(k_cvp_batch<CS, true>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
-                  : launch_cluster(k_cvp_batch<CS, false>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
+    const CvpKernelArgs& b = a;
+    return mx ? launch_cluster(k_cvp_batch<CS, false, CvpMatrixArgs>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
+         : fields ? launch_cluster(k_cvp_batch<CS, true>, b, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
+                  : launch_cluster(k_cvp_batch<CS, false>, b, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
   });
   if (e != cudaSuccess) { ctx->err = std::string("cvp batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  if ((rc = copy_matrix_out(ctx, n, mx)) != MNB_OK) return rc;
   if (!dev) {
     if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * rows, cudaMemcpyDeviceToHost, ctx->stream));
     if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * rows, cudaMemcpyDeviceToHost, ctx->stream));
@@ -844,16 +892,19 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
 
 // n full-field Dijkstra waves in one launch (k_dijkstra_batch).  The waves run in a workspace of their own, so the
 // results of the last mnb_cvp (predecessors, directions, cutting faces) and the labels of the last inflation stay valid.
+// With mx (mnb_dijkstra_matrix; no row outputs) the waves run the matrix form k_dijkstra_batch<CS, true> into mx->out.
 static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, float* out_dist,
-                                   uint32_t* out_pred) {
-  if (!ctx || !seed_vertices || (!out_dist && !out_pred) || !ctx->V || n == 0) return MNB_E_ARG;
+                                   uint32_t* out_pred, const MatrixRequest* mx = nullptr) {
+  if (!ctx || !seed_vertices || (!out_dist && !out_pred && !mx) || !ctx->V || n == 0) return MNB_E_ARG;
   if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
   for (uint32_t i = 0; i < n; ++i) if (seed_vertices[i] >= ctx->V) return MNB_INVALID_START;
-  CK(cudaSetDevice(ctx->device));
   int32_t rc;
+  if ((rc = check_targets(ctx, mx)) != MNB_OK) return rc;
+  CK(cudaSetDevice(ctx->device));
   const size_t V = ctx->V;
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
+  if (mx && !dev && (rc = ensure_out(ctx, (size_t)n * mx->m, false)) != MNB_OK) return rc;
   if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized)
     if (out_dist && (rc = ensure_out(ctx, (size_t)n * V, false)) != MNB_OK) return rc;
     if (out_pred && (size_t)n * V > ctx->batch_pred_cap) {
@@ -862,8 +913,10 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
     }
   }
   int cs = 1; unsigned groups = 1;
-  if ((rc = batch_shape(ctx, k_dijkstra_batch<1>, n, DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl), ctx->dws_groups,
-                        "Dijkstra", &cs, &groups)) != MNB_OK) return rc;
+  const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
+  rc = mx ? batch_shape(ctx, k_dijkstra_batch<1, true>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups)
+          : batch_shape(ctx, k_dijkstra_batch<1>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups);
+  if (rc != MNB_OK) return rc;
   if (groups > ctx->dws_groups) {
     dfree(ctx->dws.label); dfree(ctx->dws.mark); dfree(ctx->dws.list0); dfree(ctx->dws.list1); dfree(ctx->dws.ctl); ctx->dws_groups = 0;
     const size_t m = (size_t)groups * V;
@@ -883,14 +936,20 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
   a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
   a.next_query = ctx->d_next_query; a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V);
+  if (mx) {
+    if ((rc = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return rc;
+    a.tg.out = dev ? mx->out : ctx->d_out_dist;
+  }
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   const unsigned blocks = groups * (unsigned)cs;
   const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
     constexpr int CS = decltype(c)::value;
-    return launch_cluster(k_dijkstra_batch<CS>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
+    return mx ? launch_cluster(k_dijkstra_batch<CS, true>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
+              : launch_cluster(k_dijkstra_batch<CS>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
   });
   if (e != cudaSuccess) { ctx->err = std::string("dijkstra batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  if ((rc = copy_matrix_out(ctx, n, mx)) != MNB_OK) return rc;
   if (!dev) {
     if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
     if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1355,6 +1414,18 @@ int32_t mnb_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_vertex, d
 int32_t mnb_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, float* out_dist,
                            uint32_t* out_pred) {
   return guarded(ctx, [&]() { return impl_dijkstra_batch(ctx, n, seed_vertices, cost_limit, out_dist, out_pred); });
+}
+int32_t mnb_dijkstra_matrix(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, uint32_t m, const uint32_t* target_vertices,
+                            double cost_limit, float* out) {
+  if (!ctx || m == 0 || !target_vertices || !out) return MNB_E_ARG;
+  const MatrixRequest mx{m, target_vertices, out};
+  return guarded(ctx, [&]() { return impl_dijkstra_batch(ctx, n, seed_vertices, cost_limit, nullptr, nullptr, &mx); });
+}
+int32_t mnb_cvp_matrix(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, uint32_t m,
+                       const uint32_t* target_vertices, double cost_limit, float* out) {
+  if (!ctx || m == 0 || !target_vertices || !out) return MNB_E_ARG;
+  const MatrixRequest mx{m, target_vertices, out};
+  return guarded(ctx, [&]() { return impl_cvp_batch_fields(ctx, n, seed_faces, seed_pos, cost_limit, nullptr, nullptr, nullptr, nullptr, &mx); });
 }
 int32_t mnb_inflate(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid,
                     const mnb_inflation_params* params, float* out_dist, float* out_cost) {
