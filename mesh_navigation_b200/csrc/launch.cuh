@@ -4,8 +4,14 @@
 // this very file with g++, which has no <<<>>>.  MNB_EMU_ACTIVE is only ever defined by tests/emu/cuda_runtime.h; the
 // shipped library is built by nvcc without it and contains no host execution path for any kernel.
 #ifdef MNB_EMU_ACTIVE
+// <<<>>> converts the arguments to the kernel's parameter types (a DeviceBuffer to its pointer); the interpreter's launch
+// takes them as given, so they are converted here
+template <class... KArgs, class... Args>
+static inline cudaError_t mnb_interpreted_launch(void (*kern)(KArgs...), unsigned grid, unsigned block, size_t smem, Args&&... args) {
+  return emu::launch(kern, grid, block, smem, 1u, false, static_cast<std::decay_t<KArgs>>(std::forward<Args>(args))...);
+}
 #define MNB_LAUNCH(kern, grid, block, smem, stream, ...) \
-  emu::launch(kern, (unsigned)(grid), (unsigned)(block), (size_t)(smem), 1u, false, __VA_ARGS__)
+  mnb_interpreted_launch(kern, (unsigned)(grid), (unsigned)(block), (size_t)(smem), __VA_ARGS__)
 #define MNB_DYNAMIC_SMEM(name) unsigned char* name = emu::g_cta.dyn_smem
 #else
 #define MNB_LAUNCH(kern, grid, block, smem, stream, ...) kern<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)

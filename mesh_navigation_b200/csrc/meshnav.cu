@@ -34,58 +34,106 @@ constexpr float DIJKSTRA_BATCH_DELTA_W = 1.5f;
 // ============================================================================
 // host side
 // ============================================================================
-struct mnb_ctx {
+// One device array and its owner: a capacity in elements that only grows (reserve) and a release in the destructor.  It
+// converts to T*, so launches and copies read as with a raw pointer.  A failed reserve leaves the buffer empty (null,
+// capacity 0), never a null pointer under the capacity of the array it replaced.
+template <class T>
+struct DeviceBuffer {
+  T* p = nullptr;
+  size_t cap = 0;
+  DeviceBuffer() = default;
+  DeviceBuffer(DeviceBuffer&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DeviceBuffer& operator=(DeviceBuffer&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~DeviceBuffer() { if (p) cudaFree(p); }
+  operator T*() const { return p; }
+  cudaError_t reserve(size_t n) {
+    if (n <= cap) return cudaSuccess;
+    if (p) cudaFree(p);
+    p = nullptr; cap = 0;
+    const cudaError_t e = cudaMalloc((void**)&p, n * sizeof(T));
+    if (e == cudaSuccess) cap = n; else p = nullptr;
+    return e;
+  }
+};
+
+// Ray caster over the faces (kernels_raycast.cuh; built on first use) + state of the obstacle layer.  A default-constructed
+// value is "not built": free_raycaster assigns one.
+struct RayCasterState {
+  bool bvh_valid = false; float bvh_eps = 0.0f;
+  DeviceBuffer<float4> bvh_lo, bvh_hi; DeviceBuffer<uint32_t> bvh_parent, bvh_order; DeviceBuffer<unsigned int> bvh_visits, bvh_scene;   // the arrays of RayBvh (ray_bvh)
+  DeviceBuffer<unsigned int> d_ray_overflow;
+  DeviceBuffer<float> d_ray_in, d_ray_out;      // staging of host-pointer inputs / outputs of the ray calls
+  DeviceBuffer<uint8_t> d_obst_now, d_obst_mask; DeviceBuffer<float> d_obst_member, d_obst_member_chg;
+  DeviceBuffer<uint32_t> d_obst_list;
+};
+
+// the arrays of WaveWorkspace / DijkstraBatchWorkspace (wave_workspace, dijkstra_workspace fill the kernels' views)
+struct WaveBuffers {
+  DeviceBuffer<uint4> state, skipw;
+  DeviceBuffer<uint32_t> ext, root, pool, last_eval, dirty, chg, ver, mark, list0, list1;
+  DeviceBuffer<GroupCtl> ctl;
+};
+struct DijkstraBatchBuffers { DeviceBuffer<float> label; DeviceBuffer<uint32_t> mark, list0, list1; DeviceBuffer<GroupCtl> ctl; };
+
+// Everything that is sized by the mesh or computed from it, with the flags and counters that describe it.  A
+// default-constructed value is "no mesh": free_mesh assigns one, so a buffer declared here needs no other bookkeeping.
+struct MeshState : RayCasterState {
+  uint32_t V = 0, F = 0, E = 0;
+  size_t NC = 0, NA = 0;
+  DeviceBuffer<float> d_pos; DeviceBuffer<uint32_t> d_faces, d_edges;
+  DeviceBuffer<uint32_t> d_cor_ptr; DeviceBuffer<int4> d_cor_idx; DeviceBuffer<uint4> d_cor_eid; DeviceBuffer<uint32_t> d_face_cor;
+  DeviceBuffer<float4> d_cor_w, d_cor_wd;
+  DeviceBuffer<int4> d_ell_idx; DeviceBuffer<uint4> d_ell_eid; DeviceBuffer<float4> d_ell_w, d_ell_wd; DeviceBuffer<double4> d_ell_geo;
+  DeviceBuffer<uint32_t> d_adj_ptr, d_adj_nbr, d_adj_eid; DeviceBuffer<uint2> d_adj_nw; DeviceBuffer<uint4> d_ell_adj;
+  DeviceBuffer<float> d_edge_dist, d_edge_w, d_cost; DeviceBuffer<uint8_t> d_invalid;
+  DeviceBuffer<double> d_wsum;       // sums of install_weights (mnb_ctx::w_mean)
+  bool costs_set = false;
+  // workspace
+  uint32_t ws_groups = 0;
+  WaveBuffers ws;
+  uint32_t dws_groups = 0;       // the batched Dijkstra planner's own workspace (k_dijkstra_batch)
+  DijkstraBatchBuffers dws;
+  DeviceBuffer<uint32_t> d_batch_pred;    // its predecessor rows in host-pointer mode (and mnb_cvp_batch_fields')
+  DeviceBuffer<float> d_batch_dir;        // mnb_cvp_batch_fields' direction and cutting-face rows in host-pointer mode
+  DeviceBuffer<int32_t> d_batch_cut;
+  // scratch outputs for host-pointer mode
+  DeviceBuffer<float> d_out_dist, d_out_dir, d_out_cost; DeviceBuffer<uint32_t> d_out_pred; DeviceBuffer<int32_t> d_out_cut;
+  // target vertices of the cost-matrix calls: the caller's list and the bitmap of the distinct ones (V/32 + 1 words)
+  DeviceBuffer<uint32_t> d_targets, d_target_bits;
+  DeviceBuffer<float> d_face_normals, d_vertex_normals; DeviceBuffer<uint8_t> d_border;
+  DeviceBuffer<float> d_layer_costs, d_layer_combined, d_clearance; DeviceBuffer<uint8_t> d_layer_mask;
+  DeviceBuffer<float4> d_pos4, d_vn4; DeviceBuffer<uint32_t> d_nbr8;     // packed copies for k_layers<true>
+  DeviceBuffer<unsigned int> d_overflow;
+  // device-resident result of the last single CVP plan (for mnb_cvp_backtrack)
+  const uint32_t* last_pred = nullptr; const float* last_dir = nullptr; const int32_t* last_cut = nullptr;
+  uint32_t last_seed_face = 0; float last_seed_pos[3] = {0, 0, 0}; bool last_valid = false;
+  DeviceBuffer<float> d_path_pos; DeviceBuffer<uint32_t> d_path_face; DeviceBuffer<int32_t> d_bt_result;
+  DeviceBuffer<uint8_t> d_infl_invalid;
+  // repulsive vector field of the last inflation (InflationLayer::vector_map_ / distances_)
+  bool infl_labels_valid = false, infl_had_invalid = false, infl_field_valid = false, repulsive_on = false;
+  mnb_inflation_params infl_params{}; uint64_t infl_rounds = 0;
+  DeviceBuffer<float> d_infl_vec, d_infl_dist; DeviceBuffer<int4> d_infl_src; DeviceBuffer<unsigned int> d_infl_flag;
+  // incremental updates
+  DeviceBuffer<float> d_prev_risk; bool prev_risk_valid = false;     // riskiness map of the previous inflation (NaN = no entry)
+  DeviceBuffer<uint32_t> d_upd_ids; DeviceBuffer<float> d_upd_costs;
+  DeviceBuffer<uint32_t> d_upd_stamp; uint32_t upd_call = 0;      // change-set membership stamps of mnb_update_vertex_costs
+  DeviceBuffer<uint32_t> d_changed; DeviceBuffer<unsigned int> d_tile_count, d_total;
+};
+
+// The mesh state (replaced as a whole by mnb_set_mesh) and what lives as long as the context: stream, events, the staging
+// that is sized by a call and not by the mesh, the tuning.  Arrays one call needs and the next does not are locals of it.
+struct mnb_ctx : MeshState {
   int device = 0;
   cudaStream_t stream = nullptr;
   std::string err;
   int ptr_mode = MNB_PTR_HOST;
   int sm_count = 0;
-  // mesh
-  uint32_t V = 0, F = 0, E = 0;
-  size_t NC = 0, NA = 0;
   HostTopology topo;
-  float* d_pos = nullptr; uint32_t* d_faces = nullptr; uint32_t* d_edges = nullptr;
-  uint32_t* d_cor_ptr = nullptr; int4* d_cor_idx = nullptr; uint4* d_cor_eid = nullptr; uint32_t* d_face_cor = nullptr;
-  float4* d_cor_w = nullptr; float4* d_cor_wd = nullptr;
-  int4* d_ell_idx = nullptr; uint4* d_ell_eid = nullptr; float4* d_ell_w = nullptr; float4* d_ell_wd = nullptr; double4* d_ell_geo = nullptr;
-  uint32_t* d_adj_ptr = nullptr; uint32_t* d_adj_nbr = nullptr; uint32_t* d_adj_eid = nullptr; uint2* d_adj_nw = nullptr; uint4* d_ell_adj = nullptr;
-  float* d_edge_dist = nullptr; float* d_edge_w = nullptr; float* d_cost = nullptr; uint8_t* d_invalid = nullptr;
-  bool has_invalid = false, costs_set = false;
+  bool has_invalid = false;
   bool adj_dirty = true;       // the Dijkstra planner's weight tables (adj_nw, ell_adj) are rebuilt on its first call after new weights
-  // workspace
-  uint32_t ws_groups = 0;
-  WaveWorkspace ws{};
-  uint32_t dws_groups = 0;       // the batched Dijkstra planner's own workspace (k_dijkstra_batch)
-  DijkstraBatchWorkspace dws{};
-  uint32_t* d_batch_pred = nullptr; size_t batch_pred_cap = 0;    // its predecessor rows in host-pointer mode (and mnb_cvp_batch_fields')
-  float* d_batch_dir = nullptr; size_t batch_dir_cap = 0;         // mnb_cvp_batch_fields' direction and cutting-face rows in host-pointer mode
-  int32_t* d_batch_cut = nullptr; size_t batch_cut_cap = 0;
-  unsigned int* d_next_query = nullptr;
+  DeviceBuffer<unsigned int> d_next_query;
   int* h_cancel = nullptr; int* d_cancel = nullptr;
-  // scratch outputs for host-pointer mode
-  float* d_out_dist = nullptr; size_t out_dist_cap = 0;
-  uint32_t* d_out_pred = nullptr; float* d_out_dir = nullptr; int32_t* d_out_cut = nullptr;
-  uint32_t* d_seed_faces = nullptr; float* d_seed_pos = nullptr; uint32_t seed_cap = 0;
-  // target vertices of the cost-matrix calls: the caller's list and the bitmap of the distinct ones (V/32 + 1 words)
-  uint32_t* d_targets = nullptr; uint32_t targets_cap = 0; uint32_t* d_target_bits = nullptr;
-  float* d_face_normals = nullptr; float* d_vertex_normals = nullptr; uint8_t* d_border = nullptr;
-  float* d_layer_costs = nullptr; float* d_layer_combined = nullptr; uint8_t* d_layer_mask = nullptr; float* d_clearance = nullptr;
-  float4* d_pos4 = nullptr; float4* d_vn4 = nullptr; uint32_t* d_nbr8 = nullptr;     // packed copies for k_layers<true>
-  unsigned int* d_overflow = nullptr;
-  // device-resident result of the last single CVP plan (for mnb_cvp_backtrack)
-  const uint32_t* last_pred = nullptr; const float* last_dir = nullptr; const int32_t* last_cut = nullptr;
-  uint32_t last_seed_face = 0; float last_seed_pos[3] = {0, 0, 0}; bool last_valid = false;
-  float* d_path_pos = nullptr; uint32_t* d_path_face = nullptr; int32_t* d_bt_result = nullptr; uint32_t path_cap = 0;
-  uint32_t* d_lethals = nullptr; uint32_t lethal_cap = 0; uint8_t* d_infl_invalid = nullptr; float* d_out_cost = nullptr;
-  // repulsive vector field of the last inflation (InflationLayer::vector_map_ / distances_)
-  bool infl_labels_valid = false, infl_had_invalid = false, infl_field_valid = false, repulsive_on = false;
-  mnb_inflation_params infl_params{}; uint64_t infl_rounds = 0;
-  float* d_infl_vec = nullptr; float* d_infl_dist = nullptr; int4* d_infl_src = nullptr; unsigned int* d_infl_flag = nullptr;
-  // incremental updates
-  float* d_prev_risk = nullptr; bool prev_risk_valid = false;     // riskiness map of the previous inflation (NaN = no entry)
-  uint32_t* d_upd_ids = nullptr; float* d_upd_costs = nullptr; size_t upd_cap = 0; size_t upd_cost_cap = 0;
-  uint32_t* d_upd_stamp = nullptr; uint32_t upd_call = 0;      // change-set membership stamps of mnb_update_vertex_costs
-  uint32_t* d_changed = nullptr; unsigned int* d_tile_count = nullptr; unsigned int* d_total = nullptr;
+  DeviceBuffer<uint32_t> d_seed_faces, d_lethals; DeviceBuffer<float> d_seed_pos;
   // tuning
   float delta = 0.3f; int cluster = -1 /* -1: whole-grid cooperative kernel for single plans */; int batch_cluster = 0 /* 0: chosen per call from the goal count */; int threads = 512;
   int grid_blocks_per_sm = 0;
@@ -104,12 +152,7 @@ struct mnb_ctx {
   // Dijkstra batches (install_weights); one dependency hop is
   // ~1.35 w (the in-round sweeps are counted in hops).  On the 0.1 m bench meshes (w = 0.118) that is 0.3 / 2.4 / 3.0 m, the values
   // the kernels were tuned with.
-  bool delta_explicit = false; float w_mean = 0.0f; double* d_wsum = nullptr;
-  // ray caster over the faces (kernels_raycast.cuh; built on first use) + state of the obstacle layer
-  RayBvh bvh{}; bool bvh_valid = false; unsigned int* d_ray_overflow = nullptr;
-  float* d_ray_in = nullptr; size_t ray_in_cap = 0; float* d_ray_out = nullptr; size_t ray_out_cap = 0;
-  uint8_t* d_obst_now = nullptr; uint8_t* d_obst_mask = nullptr; float* d_obst_member = nullptr; float* d_obst_member_chg = nullptr;
-  uint32_t* d_obst_list = nullptr;
+  bool delta_explicit = false; float w_mean = 0.0f;
   mnb_stats stats{};
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 };
@@ -123,32 +166,13 @@ struct mnb_ctx {
     }                                                                              \
   } while (0)
 
-template <class T>
-static cudaError_t dalloc(T** p, size_t n) { return cudaMalloc((void**)p, n * sizeof(T) > 0 ? n * sizeof(T) : 1); }
-template <class T>
-static void dfree(T*& p) { if (p) cudaFree(p); p = nullptr; }
+static void free_raycaster(mnb_ctx* c) { static_cast<RayCasterState&>(*c) = RayCasterState{}; }
+static void free_mesh(mnb_ctx* c) { static_cast<MeshState&>(*c) = MeshState{}; }
 
-static void free_raycaster(mnb_ctx* c);
-static void free_mesh(mnb_ctx* c) {
-  free_raycaster(c);
-  dfree(c->d_pos); dfree(c->d_faces); dfree(c->d_edges); dfree(c->d_cor_ptr); dfree(c->d_cor_idx); dfree(c->d_cor_eid); dfree(c->d_face_cor);
-  dfree(c->d_cor_w); dfree(c->d_cor_wd); dfree(c->d_ell_idx); dfree(c->d_ell_eid); dfree(c->d_ell_w); dfree(c->d_ell_wd); dfree(c->d_ell_geo); dfree(c->d_adj_ptr); dfree(c->d_adj_nbr); dfree(c->d_adj_eid); dfree(c->d_adj_nw); dfree(c->d_ell_adj);
-  dfree(c->d_edge_dist); dfree(c->d_edge_w); dfree(c->d_cost); dfree(c->d_invalid); dfree(c->d_wsum);
-  dfree(c->ws.state); dfree(c->ws.ext); dfree(c->ws.pool); dfree(c->ws.skipw); dfree(c->ws.root); dfree(c->ws.last_eval); dfree(c->ws.dirty); dfree(c->ws.chg); dfree(c->ws.ver); dfree(c->ws.mark); dfree(c->ws.list0); dfree(c->ws.list1); dfree(c->ws.ctl);
-  c->ws_groups = 0;
-  dfree(c->dws.label); dfree(c->dws.mark); dfree(c->dws.list0); dfree(c->dws.list1); dfree(c->dws.ctl); c->dws_groups = 0;
-  dfree(c->d_batch_pred); c->batch_pred_cap = 0; dfree(c->d_batch_dir); c->batch_dir_cap = 0; dfree(c->d_batch_cut); c->batch_cut_cap = 0;
-  dfree(c->d_out_dist); c->out_dist_cap = 0; dfree(c->d_out_pred); dfree(c->d_out_dir); dfree(c->d_out_cut);
-  dfree(c->d_targets); c->targets_cap = 0; dfree(c->d_target_bits);
-  dfree(c->d_infl_invalid); dfree(c->d_out_cost);
-  dfree(c->d_infl_vec); dfree(c->d_infl_dist); dfree(c->d_infl_src); dfree(c->d_infl_flag);
-  c->infl_labels_valid = false; c->infl_field_valid = false; c->repulsive_on = false;
-  dfree(c->d_prev_risk); c->prev_risk_valid = false; dfree(c->d_upd_ids); dfree(c->d_upd_costs); c->upd_cap = 0; c->upd_cost_cap = 0; dfree(c->d_upd_stamp); c->upd_call = 0;
-  dfree(c->d_changed); dfree(c->d_tile_count); dfree(c->d_total);
-  dfree(c->d_path_pos); dfree(c->d_path_face); dfree(c->d_bt_result); c->path_cap = 0; c->last_valid = false;
-  dfree(c->d_face_normals); dfree(c->d_vertex_normals); dfree(c->d_border); dfree(c->d_layer_costs); dfree(c->d_layer_combined);
-  dfree(c->d_layer_mask); dfree(c->d_clearance); dfree(c->d_overflow); dfree(c->d_pos4); dfree(c->d_vn4); dfree(c->d_nbr8);
-  c->costs_set = false;
+// stats of a call that is not a wavefront (finish_stats): the time between ev0 and ev1, once the stream has synchronised
+static void simple_stats(mnb_ctx* ctx, uint64_t launches, uint64_t settled) {
+  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = launches; ctx->stats.settled = settled;
 }
 
 // level pool (band_engine.cuh): pop times with more than 3 cascade levels keep their tails here; 2 words per vertex
@@ -162,15 +186,31 @@ static size_t ws_bytes_per_group(uint32_t V) {
 
 static int32_t ensure_workspace(mnb_ctx* ctx, uint32_t groups) {
   if (groups <= ctx->ws_groups) return MNB_OK;
-  dfree(ctx->ws.state); dfree(ctx->ws.ext); dfree(ctx->ws.pool); dfree(ctx->ws.skipw); dfree(ctx->ws.root); dfree(ctx->ws.last_eval); dfree(ctx->ws.dirty); dfree(ctx->ws.chg); dfree(ctx->ws.ver); dfree(ctx->ws.mark); dfree(ctx->ws.list0); dfree(ctx->ws.list1); dfree(ctx->ws.ctl);
+  WaveBuffers& w = ctx->ws;
+  w = WaveBuffers{};         // the smaller workspace goes first: batch_shape has counted its bytes as available
   ctx->ws_groups = 0;
-  const size_t n = (size_t)groups * ctx->V;
-  CK(dalloc(&ctx->ws.state, n)); CK(dalloc(&ctx->ws.ext, n)); CK(dalloc(&ctx->ws.skipw, n)); CK(dalloc(&ctx->ws.root, n)); CK(dalloc(&ctx->ws.last_eval, (size_t)ctx->V)); CK(dalloc(&ctx->ws.dirty, (size_t)ctx->V)); CK(dalloc(&ctx->ws.chg, n)); CK(dalloc(&ctx->ws.ver, (size_t)ctx->V)); CK(dalloc(&ctx->ws.mark, n)); CK(dalloc(&ctx->ws.list0, n)); CK(dalloc(&ctx->ws.list1, n));
-  ctx->ws.pool_cap = ws_pool_cap(ctx->V);
-  CK(dalloc(&ctx->ws.pool, (size_t)groups * ctx->ws.pool_cap));
-  CK(dalloc(&ctx->ws.ctl, groups));
+  const size_t n = (size_t)groups * ctx->V, V = ctx->V;
+  CK(w.state.reserve(n)); CK(w.ext.reserve(n)); CK(w.skipw.reserve(n)); CK(w.root.reserve(n)); CK(w.last_eval.reserve(V)); CK(w.dirty.reserve(V)); CK(w.chg.reserve(n)); CK(w.ver.reserve(V)); CK(w.mark.reserve(n)); CK(w.list0.reserve(n)); CK(w.list1.reserve(n));
+  CK(w.pool.reserve((size_t)groups * ws_pool_cap(ctx->V)));
+  CK(w.ctl.reserve(groups));
   ctx->ws_groups = groups;
   return MNB_OK;
+}
+
+// the kernels' views of the workspaces: plain structs of raw pointers, passed by value
+static WaveWorkspace wave_workspace(const mnb_ctx* ctx) {
+  const WaveBuffers& b = ctx->ws;
+  WaveWorkspace w{};
+  w.state = b.state; w.ext = b.ext; w.root = b.root; w.pool = b.pool; w.pool_cap = ws_pool_cap(ctx->V);
+  w.last_eval = b.last_eval; w.dirty = b.dirty; w.skipw = b.skipw; w.chg = b.chg; w.ver = b.ver;
+  w.mark = b.mark; w.list0 = b.list0; w.list1 = b.list1; w.ctl = b.ctl;
+  return w;
+}
+static DijkstraBatchWorkspace dijkstra_workspace(const mnb_ctx* ctx) {
+  const DijkstraBatchBuffers& b = ctx->dws;
+  DijkstraBatchWorkspace w{};
+  w.label = b.label; w.mark = b.mark; w.list0 = b.list0; w.list1 = b.list1; w.ctl = b.ctl;
+  return w;
 }
 
 // Runs the body of a C-ABI entry point: std::bad_alloc (the host tables of a 50M-vertex map are tens of GB) becomes
@@ -207,7 +247,7 @@ int32_t mnb_create(int32_t device, mnb_ctx** out_ctx) {
   c->device = device; c->sm_count = prop.multiProcessorCount;
   if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return MNB_E_CUDA; }
   cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
-  cudaMalloc((void**)&c->d_next_query, sizeof(unsigned int));
+  c->d_next_query.reserve(1);
   if (cudaHostAlloc((void**)&c->h_cancel, sizeof(int), cudaHostAllocMapped) == cudaSuccess) {
     *c->h_cancel = 0;
     cudaHostGetDevicePointer((void**)&c->d_cancel, c->h_cancel, 0);
@@ -220,8 +260,6 @@ void mnb_destroy(mnb_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  free_mesh(ctx);
-  dfree(ctx->d_next_query); dfree(ctx->d_seed_faces); dfree(ctx->d_seed_pos); dfree(ctx->d_lethals);
   if (ctx->h_cancel) cudaFreeHost(ctx->h_cancel);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -282,12 +320,12 @@ static int32_t impl_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* 
   }
   ctx->V = V; ctx->F = F; ctx->E = T.E; ctx->NC = T.cor_v1.size(); ctx->NA = T.vadj_nbr.size();
   const size_t NC = ctx->NC, NA = ctx->NA;
-  CK(dalloc(&ctx->d_pos, 3 * (size_t)V)); CK(dalloc(&ctx->d_faces, 3 * (size_t)F)); CK(dalloc(&ctx->d_edges, 2 * (size_t)T.E));
-  CK(dalloc(&ctx->d_cor_ptr, (size_t)V + 1)); CK(dalloc(&ctx->d_cor_idx, NC)); CK(dalloc(&ctx->d_cor_eid, NC));
-  CK(dalloc(&ctx->d_cor_w, NC)); CK(dalloc(&ctx->d_cor_wd, NC));
-  CK(dalloc(&ctx->d_adj_ptr, (size_t)V + 1)); CK(dalloc(&ctx->d_adj_nbr, NA)); CK(dalloc(&ctx->d_adj_eid, NA)); CK(dalloc(&ctx->d_adj_nw, NA)); CK(dalloc(&ctx->d_ell_adj, (size_t)V * ELL_W));
-  CK(dalloc(&ctx->d_edge_dist, (size_t)T.E)); CK(dalloc(&ctx->d_edge_w, (size_t)T.E)); CK(dalloc(&ctx->d_cost, (size_t)V));
-  CK(dalloc(&ctx->d_invalid, (size_t)V));
+  CK(ctx->d_pos.reserve(3 * (size_t)V)); CK(ctx->d_faces.reserve(3 * (size_t)F)); CK(ctx->d_edges.reserve(2 * (size_t)T.E));
+  CK(ctx->d_cor_ptr.reserve((size_t)V + 1)); CK(ctx->d_cor_idx.reserve(NC)); CK(ctx->d_cor_eid.reserve(NC));
+  CK(ctx->d_cor_w.reserve(NC)); CK(ctx->d_cor_wd.reserve(NC));
+  CK(ctx->d_adj_ptr.reserve((size_t)V + 1)); CK(ctx->d_adj_nbr.reserve(NA)); CK(ctx->d_adj_eid.reserve(NA)); CK(ctx->d_adj_nw.reserve(NA)); CK(ctx->d_ell_adj.reserve((size_t)V * ELL_W));
+  CK(ctx->d_edge_dist.reserve((size_t)T.E)); CK(ctx->d_edge_w.reserve((size_t)T.E)); CK(ctx->d_cost.reserve((size_t)V));
+  CK(ctx->d_invalid.reserve((size_t)V));
   CK(cudaMemcpyAsync(ctx->d_pos, pos, sizeof(float) * 3 * (size_t)V, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(ctx->d_faces, faces, sizeof(uint32_t) * 3 * (size_t)F, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(ctx->d_edges, T.edges.data(), sizeof(uint32_t) * 2 * (size_t)T.E, cudaMemcpyHostToDevice, ctx->stream));
@@ -303,7 +341,7 @@ static int32_t impl_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* 
     }
     CK(cudaMemcpyAsync(ctx->d_cor_idx, idx.data(), sizeof(int4) * NC, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_cor_eid, eid.data(), sizeof(uint4) * NC, cudaMemcpyHostToDevice, ctx->stream));
-    CK(dalloc(&ctx->d_face_cor, 3 * (size_t)F));
+    CK(ctx->d_face_cor.reserve(3 * (size_t)F));
     CK(cudaMemcpyAsync(ctx->d_face_cor, T.face_cor.data(), sizeof(uint32_t) * 3 * (size_t)F, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     // ELL rows: 8 slots per vertex (one 128-byte line), slot 0 carries the degree in .w
@@ -314,8 +352,8 @@ static int32_t impl_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* 
       for (uint32_t k = kb; k < ke && k - kb < ELL_W; ++k) { eidx[(size_t)v * ELL_W + (k - kb)] = idx[k]; eeid[(size_t)v * ELL_W + (k - kb)] = eid[k]; }
       eidx[(size_t)v * ELL_W].w = (int)(ke - kb);
     }
-    CK(dalloc(&ctx->d_ell_idx, NE)); CK(dalloc(&ctx->d_ell_eid, NE)); CK(dalloc(&ctx->d_ell_w, NE)); CK(dalloc(&ctx->d_ell_wd, NE));
-    CK(dalloc(&ctx->d_ell_geo, NE));
+    CK(ctx->d_ell_idx.reserve(NE)); CK(ctx->d_ell_eid.reserve(NE)); CK(ctx->d_ell_w.reserve(NE)); CK(ctx->d_ell_wd.reserve(NE));
+    CK(ctx->d_ell_geo.reserve(NE));
     CK(cudaMemcpyAsync(ctx->d_ell_idx, eidx.data(), sizeof(int4) * NE, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_ell_eid, eeid.data(), sizeof(uint4) * NE, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -325,7 +363,7 @@ static int32_t impl_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* 
   std::vector<uint32_t>().swap(T.cor_ec); std::vector<uint32_t>().swap(T.cor_eb); std::vector<uint32_t>().swap(T.cor_ea);
   std::vector<uint8_t>().swap(T.cor_side);
   std::vector<uint32_t>().swap(T.vadj_nbr); std::vector<uint32_t>().swap(T.vadj_eid); std::vector<uint32_t>().swap(T.face_edges);
-  CK(dalloc(&ctx->d_face_normals, 3 * (size_t)F)); CK(dalloc(&ctx->d_vertex_normals, 3 * (size_t)V)); CK(dalloc(&ctx->d_border, (size_t)V));
+  CK(ctx->d_face_normals.reserve(3 * (size_t)F)); CK(ctx->d_vertex_normals.reserve(3 * (size_t)V)); CK(ctx->d_border.reserve((size_t)V));
   CK(cudaMemcpyAsync(ctx->d_border, T.border.data(), (size_t)V, cudaMemcpyHostToDevice, ctx->stream));
   MNB_LAUNCH(k_face_normals, (F + 255) / 256, 256, 0, ctx->stream, ctx->d_pos, ctx->d_faces, F, ctx->d_face_normals);
   MNB_LAUNCH(k_vertex_normals, (V + 255) / 256, 256, 0, ctx->stream, ctx->d_cor_ptr, ctx->d_cor_idx, ctx->d_face_normals, V, ctx->d_vertex_normals);
@@ -361,7 +399,7 @@ static int32_t install_weights(mnb_ctx* ctx) {
   ctx->adj_dirty = true;        // adjacency form of the weights: only the Dijkstra planner reads it (ensure_adj_tables)
   CK(cudaGetLastError());
   // scale of the potentials: mean finite edge weight (see mnb_ctx::delta_explicit)
-  if (!ctx->d_wsum) CK(dalloc(&ctx->d_wsum, 2));
+  CK(ctx->d_wsum.reserve(2));
   CK(cudaMemsetAsync(ctx->d_wsum, 0, 2 * sizeof(double), ctx->stream));
   MNB_LAUNCH(k_weight_scale, 2 * ctx->sm_count, 256, 0, ctx->stream, (const float*)ctx->d_edge_w, ctx->E, ctx->d_wsum);
   CK(cudaGetLastError());
@@ -450,10 +488,10 @@ static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
   }
   CK(cudaSetDevice(ctx->device));
   const size_t V = ctx->V;
-  if (!ctx->d_infl_vec) { CK(dalloc(&ctx->d_infl_vec, 3 * V)); CK(dalloc(&ctx->d_infl_src, V)); CK(dalloc(&ctx->d_infl_flag, (size_t)2)); }
+  CK(ctx->d_infl_vec.reserve(3 * V)); CK(ctx->d_infl_src.reserve(V)); CK(ctx->d_infl_flag.reserve(2));
   InflVecArgs a{};
   a.V = ctx->V; a.pos = ctx->d_pos; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx; a.cor_wd = ctx->d_cor_wd;
-  a.cor_eid = ctx->d_cor_eid; a.adj_ptr = ctx->d_adj_ptr; a.adj_nbr = ctx->d_adj_nbr; a.invalid = ctx->infl_had_invalid ? ctx->d_infl_invalid : nullptr; a.ws = ctx->ws;
+  a.cor_eid = ctx->d_cor_eid; a.adj_ptr = ctx->d_adj_ptr; a.adj_nbr = ctx->d_adj_nbr; a.invalid = ctx->infl_had_invalid ? ctx->d_infl_invalid.p : nullptr; a.ws = wave_workspace(ctx);
   a.max_distance = (float)ctx->infl_params.inflation_radius; a.vec = ctx->d_infl_vec; a.src = ctx->d_infl_src; a.flag = ctx->d_infl_flag;
   CK(cudaMemsetAsync(ctx->d_infl_flag, 0, 2 * sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
@@ -476,9 +514,8 @@ static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
   if (flag[0]) { ctx->err = "inflation vector field did not reach its fixed point"; return MNB_E_STATE; }
   if (out_vectors) CK(cudaMemcpyAsync(out_vectors, ctx->d_infl_vec, sizeof(float) * 3 * V, out_kind(ctx), ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  const uint64_t wave_rounds = ctx->infl_rounds;
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = launches; ctx->stats.settled = ctx->V; ctx->stats.rounds = wave_rounds;
+  simple_stats(ctx, launches, ctx->V);
+  ctx->stats.rounds = ctx->infl_rounds;
   ctx->infl_field_valid = true;
   return MNB_OK;
 }
@@ -496,9 +533,9 @@ static int32_t impl_inflation_vector_at(mnb_ctx* ctx, uint32_t n, const uint32_t
   for (uint32_t i = 0; ctx->ptr_mode == MNB_PTR_HOST && i < n; ++i) if (faces_q[i] >= ctx->F) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  uint32_t* d_f = nullptr; float* d_b = nullptr; float* d_o = nullptr;
+  DeviceBuffer<uint32_t> d_f; DeviceBuffer<float> d_b, d_o;      // host-pointer mode: device copies for this call
   if (!dev) {
-    CK(dalloc(&d_f, (size_t)n)); CK(dalloc(&d_b, 3 * (size_t)n)); CK(dalloc(&d_o, 3 * (size_t)n));
+    CK(d_f.reserve((size_t)n)); CK(d_b.reserve(3 * (size_t)n)); CK(d_o.reserve(3 * (size_t)n));
     CK(cudaMemcpyAsync(d_f, faces_q, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_b, bary, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   }
@@ -507,7 +544,6 @@ static int32_t impl_inflation_vector_at(mnb_ctx* ctx, uint32_t n, const uint32_t
   CK(cudaGetLastError());
   if (!dev) CK(cudaMemcpyAsync(out, d_o, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  dfree(d_f); dfree(d_b); dfree(d_o);
   return MNB_OK;
 }
 
@@ -614,19 +650,13 @@ static int32_t finish_stats(mnb_ctx* ctx, unsigned groups, unsigned launches, co
 }
 
 static int32_t ensure_out(mnb_ctx* ctx, size_t n_dist, bool aux) {
-  if (n_dist > ctx->out_dist_cap) { dfree(ctx->d_out_dist); CK(dalloc(&ctx->d_out_dist, n_dist)); ctx->out_dist_cap = n_dist; }
-  if (aux && !ctx->d_out_pred) {
-    CK(dalloc(&ctx->d_out_pred, (size_t)ctx->V)); CK(dalloc(&ctx->d_out_dir, (size_t)ctx->V)); CK(dalloc(&ctx->d_out_cut, (size_t)ctx->V));
-  }
+  CK(ctx->d_out_dist.reserve(n_dist));
+  if (aux) { CK(ctx->d_out_pred.reserve(ctx->V)); CK(ctx->d_out_dir.reserve(ctx->V)); CK(ctx->d_out_cut.reserve(ctx->V)); }
   return MNB_OK;
 }
 
 static int32_t ensure_seeds(mnb_ctx* ctx, uint32_t n) {
-  if (n > ctx->seed_cap) {
-    dfree(ctx->d_seed_faces); dfree(ctx->d_seed_pos);
-    CK(dalloc(&ctx->d_seed_faces, (size_t)n)); CK(dalloc(&ctx->d_seed_pos, 3 * (size_t)n));
-    ctx->seed_cap = n;
-  }
+  CK(ctx->d_seed_faces.reserve(n)); CK(ctx->d_seed_pos.reserve(3 * (size_t)n));
   return MNB_OK;
 }
 
@@ -642,8 +672,7 @@ static int32_t check_targets(mnb_ctx* ctx, const MatrixRequest* mx) {
 // Uploads the target list and the bitmap of the distinct targets (ctx buffers, freed with the mesh) and fills tg but out.
 static int32_t upload_targets(mnb_ctx* ctx, const MatrixRequest& mx, TargetSet& tg) {
   const size_t words = ((size_t)ctx->V >> 5) + 1;
-  if (!ctx->d_target_bits) CK(dalloc(&ctx->d_target_bits, words));
-  if (mx.m > ctx->targets_cap) { dfree(ctx->d_targets); ctx->targets_cap = 0; CK(dalloc(&ctx->d_targets, (size_t)mx.m)); ctx->targets_cap = mx.m; }
+  CK(ctx->d_target_bits.reserve(words)); CK(ctx->d_targets.reserve(mx.m));
   std::vector<uint32_t> bits(words, 0u);     // (a copy from pageable memory has read it when cudaMemcpyAsync returns)
   uint32_t distinct = 0;
   for (uint32_t j = 0; j < mx.m; ++j) {
@@ -665,7 +694,7 @@ static int32_t copy_matrix_out(mnb_ctx* ctx, uint32_t n, const MatrixRequest* mx
 
 static void fill_cvp_args(mnb_ctx* ctx, CvpKernelArgs& a) {
   a.V = ctx->V; a.pos = ctx->d_pos; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx;
-  a.cor_w = ctx->d_cor_w; a.ell_idx = ctx->d_ell_idx; a.ell_w = ctx->d_ell_w; a.ell_geo = ctx->d_ell_geo; a.cost = ctx->d_cost; a.invalid = ctx->has_invalid ? ctx->d_invalid : nullptr; a.ws = ctx->ws;
+  a.cor_w = ctx->d_cor_w; a.ell_idx = ctx->d_ell_idx; a.ell_w = ctx->d_ell_w; a.ell_geo = ctx->d_ell_geo; a.cost = ctx->d_cost; a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = wave_workspace(ctx);
   a.seed_faces = ctx->d_seed_faces; a.seed_pos = ctx->d_seed_pos; a.delta = ctx->delta; a.next_query = ctx->d_next_query;
   a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V); a.sweeps = 0;
   a.hop = ctx->w_mean > 0 ? 1.35f * ctx->w_mean : 0.16f;
@@ -771,18 +800,9 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
   if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized; the
                        // single plan's outputs stay untouched for mnb_cvp_backtrack / mnb_vector_map)
     if (out_dist && (rc = ensure_out(ctx, rows, false)) != MNB_OK) return rc;
-    if (out_pred && rows > ctx->batch_pred_cap) {
-      dfree(ctx->d_batch_pred); ctx->batch_pred_cap = 0;
-      CK(dalloc(&ctx->d_batch_pred, rows)); ctx->batch_pred_cap = rows;
-    }
-    if (out_dir && rows > ctx->batch_dir_cap) {
-      dfree(ctx->d_batch_dir); ctx->batch_dir_cap = 0;
-      CK(dalloc(&ctx->d_batch_dir, rows)); ctx->batch_dir_cap = rows;
-    }
-    if (out_cut && rows > ctx->batch_cut_cap) {
-      dfree(ctx->d_batch_cut); ctx->batch_cut_cap = 0;
-      CK(dalloc(&ctx->d_batch_cut, rows)); ctx->batch_cut_cap = rows;
-    }
+    if (out_pred) CK(ctx->d_batch_pred.reserve(rows));
+    if (out_dir) CK(ctx->d_batch_dir.reserve(rows));
+    if (out_cut) CK(ctx->d_batch_cut.reserve(rows));
   }
   int cs = 1; unsigned groups = 1;
   rc = mx ? batch_shape(ctx, k_cvp_batch<1, false, CvpMatrixArgs>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
@@ -847,7 +867,7 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
   DijkstraKernelArgs a{};
   a.V = ctx->V; a.adj_ptr = ctx->d_adj_ptr; a.adj_nw = ctx->d_adj_nw; a.cost = ctx->d_cost;
-  a.invalid = ctx->has_invalid ? ctx->d_invalid : nullptr; a.ws = ctx->ws; a.seed_vertex = seed_vertex;
+  a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = wave_workspace(ctx); a.seed_vertex = seed_vertex;
   a.robot_vertex = robot_vertex; a.cost_limit = cost_limit; a.goal_dist_offset = goal_dist_offset; a.delta = ctx->delta;
   a.out_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist;
   a.out_pred = (dev && out_pred) ? out_pred : ctx->d_out_pred;
@@ -907,10 +927,7 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   if (mx && !dev && (rc = ensure_out(ctx, (size_t)n * mx->m, false)) != MNB_OK) return rc;
   if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized)
     if (out_dist && (rc = ensure_out(ctx, (size_t)n * V, false)) != MNB_OK) return rc;
-    if (out_pred && (size_t)n * V > ctx->batch_pred_cap) {
-      dfree(ctx->d_batch_pred); ctx->batch_pred_cap = 0;
-      CK(dalloc(&ctx->d_batch_pred, (size_t)n * V)); ctx->batch_pred_cap = (size_t)n * V;
-    }
+    if (out_pred) CK(ctx->d_batch_pred.reserve((size_t)n * V));
   }
   int cs = 1; unsigned groups = 1;
   const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
@@ -918,10 +935,11 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
           : batch_shape(ctx, k_dijkstra_batch<1>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups);
   if (rc != MNB_OK) return rc;
   if (groups > ctx->dws_groups) {
-    dfree(ctx->dws.label); dfree(ctx->dws.mark); dfree(ctx->dws.list0); dfree(ctx->dws.list1); dfree(ctx->dws.ctl); ctx->dws_groups = 0;
+    ctx->dws = DijkstraBatchBuffers{};        // the smaller workspace goes first: batch_shape has counted its bytes as available
+    ctx->dws_groups = 0;
     const size_t m = (size_t)groups * V;
-    CK(dalloc(&ctx->dws.label, m)); CK(dalloc(&ctx->dws.mark, m)); CK(dalloc(&ctx->dws.list0, m)); CK(dalloc(&ctx->dws.list1, m));
-    CK(dalloc(&ctx->dws.ctl, groups));
+    CK(ctx->dws.label.reserve(m)); CK(ctx->dws.mark.reserve(m)); CK(ctx->dws.list0.reserve(m)); CK(ctx->dws.list1.reserve(m));
+    CK(ctx->dws.ctl.reserve(groups));
     ctx->dws_groups = groups;
   }
   if (ctx->h_cancel) *ctx->h_cancel = 0;     // dijkstra:238
@@ -931,7 +949,7 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   CK(cudaMemsetAsync(ctx->dws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
   DijkstraBatchArgs a{};
   a.V = ctx->V; a.adj_ptr = ctx->d_adj_ptr; a.adj_nw = ctx->d_adj_nw; a.cost = ctx->d_cost;
-  a.invalid = ctx->has_invalid ? ctx->d_invalid : nullptr; a.ws = ctx->dws;
+  a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = dijkstra_workspace(ctx);
   a.n_queries = n; a.seeds = ctx->d_seed_faces; a.cost_limit = cost_limit; a.delta = ctx->dijkstra_batch_delta;
   a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
   a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
@@ -972,19 +990,17 @@ static int32_t impl_compute_layers(mnb_ctx* ctx, const mnb_layer_params* params,
   if (!ctx || !params || !ctx->V) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
   const size_t V = ctx->V;
-  if (!ctx->d_layer_costs) {
-    CK(dalloc(&ctx->d_layer_costs, 6 * V)); CK(dalloc(&ctx->d_layer_combined, V)); CK(dalloc(&ctx->d_layer_mask, V));
-    CK(dalloc(&ctx->d_overflow, (size_t)1));
-  }
+  CK(ctx->d_layer_costs.reserve(6 * V)); CK(ctx->d_layer_combined.reserve(V)); CK(ctx->d_layer_mask.reserve(V));
+  CK(ctx->d_overflow.reserve(1));
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   if (clearance) {
-    if (!ctx->d_clearance) CK(dalloc(&ctx->d_clearance, V));
+    CK(ctx->d_clearance.reserve(V));
     CK(cudaMemcpyAsync(ctx->d_clearance, clearance, sizeof(float) * V, in_kind(ctx), ctx->stream));
   }
   CK(cudaMemsetAsync(ctx->d_overflow, 0, sizeof(unsigned int), ctx->stream));
   LayerKernelArgs a{};
   a.V = ctx->V; a.pos = ctx->d_pos; a.vn = ctx->d_vertex_normals; a.adj_ptr = ctx->d_adj_ptr; a.adj_nbr = ctx->d_adj_nbr;
-  a.border = ctx->d_border; a.clearance = clearance ? ctx->d_clearance : nullptr; a.P = *params;
+  a.border = ctx->d_border; a.clearance = clearance ? ctx->d_clearance.p : nullptr; a.P = *params;
   a.costs = (dev && out_costs) ? out_costs : ctx->d_layer_costs;
   a.combined = (dev && out_combined) ? out_combined : ctx->d_layer_combined;
   a.lethal_mask = (dev && out_lethal_mask) ? out_lethal_mask : ctx->d_layer_mask;
@@ -992,12 +1008,12 @@ static int32_t impl_compute_layers(mnb_ctx* ctx, const mnb_layer_params* params,
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   if (ctx->layers_smem) {
     if (!ctx->d_pos4) {
-      CK(dalloc(&ctx->d_pos4, V)); CK(dalloc(&ctx->d_vn4, V)); CK(dalloc(&ctx->d_nbr8, 8 * V));
+      CK(ctx->d_pos4.reserve(V)); CK(ctx->d_vn4.reserve(V)); CK(ctx->d_nbr8.reserve(8 * V));
       MNB_LAUNCH(k_pack_layers, (ctx->V + 255) / 256, 256, 0, ctx->stream, (const float*)ctx->d_pos, (const float*)ctx->d_vertex_normals,
                  (const uint32_t*)ctx->d_adj_ptr, (const uint32_t*)ctx->d_adj_nbr, ctx->V, ctx->d_pos4, ctx->d_vn4, ctx->d_nbr8);
       CK(cudaGetLastError());
     }
-    a.pos4 = ctx->d_pos4; a.vn4 = ctx->d_vn4; a.nbr8 = reinterpret_cast<const uint4*>(ctx->d_nbr8);
+    a.pos4 = ctx->d_pos4; a.vn4 = ctx->d_vn4; a.nbr8 = reinterpret_cast<const uint4*>(ctx->d_nbr8.p);
     if (ctx->layers_smem == 8 || ctx->layers_smem == 9) {      // walk_pf16 compiled for more resident CTAs (fewer registers): 8 -> 64 x 12, 9 -> 128 x 6
       const int T = ctx->layers_smem == 8 ? 64 : 128;
       const size_t smem = (size_t)(2 * NB_HASH + LS_STACK) * T;
@@ -1035,8 +1051,7 @@ static int32_t impl_compute_layers(mnb_ctx* ctx, const mnb_layer_params* params,
   unsigned int ovf = 0;
   CK(cudaMemcpyAsync(&ovf, ctx->d_overflow, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = 1; ctx->stats.settled = ctx->V;
+  simple_stats(ctx, 1, ctx->V);
   if (ovf) { ctx->err = "layer neighbourhood exceeds the per-vertex scratch (radius too large for the mesh resolution)"; return MNB_E_NOMEM; }
   return MNB_OK;
 }
@@ -1048,16 +1063,16 @@ static int32_t impl_vector_map(mnb_ctx* ctx, const uint32_t* pred, const float* 
   const size_t V = ctx->V;
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   const uint32_t* d_pred = pred; const float* d_dir = direction; const int32_t* d_cut = cutting_face; float* d_out = out_vec;
-  float* tmp_out = nullptr; uint32_t* tmp_pred = nullptr; float* tmp_dir = nullptr; int32_t* tmp_cut = nullptr;
+  DeviceBuffer<float> tmp_out, tmp_dir; DeviceBuffer<uint32_t> tmp_pred; DeviceBuffer<int32_t> tmp_cut;
   if (!pred) {            // the device-resident result of the last CVP plan (nothing is uploaded)
     d_pred = ctx->last_pred; d_dir = ctx->last_dir; d_cut = ctx->last_cut;
-    if (!dev) { CK(dalloc(&tmp_out, 3 * V)); d_out = tmp_out; }
+    if (!dev) { CK(tmp_out.reserve(3 * V)); d_out = tmp_out; }
   } else if (!dev) {
-    CK(dalloc(&tmp_out, 3 * V)); CK(dalloc(&tmp_pred, V));
+    CK(tmp_out.reserve(3 * V)); CK(tmp_pred.reserve(V));
     CK(cudaMemcpyAsync(tmp_pred, pred, sizeof(uint32_t) * V, cudaMemcpyHostToDevice, ctx->stream));
     d_pred = tmp_pred; d_out = tmp_out;
-    if (direction) { CK(dalloc(&tmp_dir, V)); CK(cudaMemcpyAsync(tmp_dir, direction, sizeof(float) * V, cudaMemcpyHostToDevice, ctx->stream)); d_dir = tmp_dir; }
-    if (cutting_face) { CK(dalloc(&tmp_cut, V)); CK(cudaMemcpyAsync(tmp_cut, cutting_face, sizeof(int32_t) * V, cudaMemcpyHostToDevice, ctx->stream)); d_cut = tmp_cut; }
+    if (direction) { CK(tmp_dir.reserve(V)); CK(cudaMemcpyAsync(tmp_dir, direction, sizeof(float) * V, cudaMemcpyHostToDevice, ctx->stream)); d_dir = tmp_dir; }
+    if (cutting_face) { CK(tmp_cut.reserve(V)); CK(cudaMemcpyAsync(tmp_cut, cutting_face, sizeof(int32_t) * V, cudaMemcpyHostToDevice, ctx->stream)); d_cut = tmp_cut; }
   }
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   MNB_LAUNCH(k_vector_map, (ctx->V + 255) / 256, 256, 0, ctx->stream, ctx->d_pos, ctx->d_vertex_normals, d_pred, d_dir, d_cut, ctx->V, d_out);
@@ -1065,9 +1080,7 @@ static int32_t impl_vector_map(mnb_ctx* ctx, const uint32_t* pred, const float* 
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (!dev) CK(cudaMemcpyAsync(out_vec, d_out, sizeof(float) * 3 * V, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  dfree(tmp_out); dfree(tmp_pred); dfree(tmp_dir); dfree(tmp_cut);
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = 1; ctx->stats.settled = ctx->V;
+  simple_stats(ctx, 1, ctx->V);
   return MNB_OK;
 }
 
@@ -1077,12 +1090,8 @@ static int32_t impl_cvp_backtrack(mnb_ctx* ctx, const float robot_pos[3], uint32
   if (!ctx->last_valid) { ctx->err = "mnb_cvp_backtrack needs a preceding successful mnb_cvp on this context"; return MNB_E_STATE; }
   if (robot_face >= ctx->F) return MNB_INVALID_GOAL;
   CK(cudaSetDevice(ctx->device));
-  if (max_points > ctx->path_cap) {
-    dfree(ctx->d_path_pos); dfree(ctx->d_path_face); ctx->path_cap = 0;
-    CK(dalloc(&ctx->d_path_pos, 3 * (size_t)max_points)); CK(dalloc(&ctx->d_path_face, (size_t)max_points));
-    ctx->path_cap = max_points;
-  }
-  if (!ctx->d_bt_result) CK(dalloc(&ctx->d_bt_result, (size_t)2));
+  CK(ctx->d_path_pos.reserve(3 * (size_t)max_points)); CK(ctx->d_path_face.reserve(max_points));
+  CK(ctx->d_bt_result.reserve(2));
   BacktrackArgs a{};
   a.pos = ctx->d_pos; a.vn = ctx->d_vertex_normals; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx;
   a.pred = ctx->last_pred; a.direction = ctx->last_dir; a.cut = ctx->last_cut;
@@ -1105,8 +1114,7 @@ static int32_t impl_cvp_backtrack(mnb_ctx* ctx, const float robot_pos[3], uint32
   CK(cudaMemcpyAsync(path_pos, ctx->d_path_pos, sizeof(float) * 3 * (size_t)n, kind, ctx->stream));
   if (path_face) CK(cudaMemcpyAsync(path_face, ctx->d_path_face, sizeof(uint32_t) * (size_t)n, kind, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = 1; ctx->stats.settled = n;
+  simple_stats(ctx, 1, n);
   if (res[0] == MNB_E_STATE) { ctx->err = "back-tracking exceeded max_points (cyclic vector field?) or the face search list"; return MNB_E_STATE; }
   return res[0];
 }
@@ -1115,12 +1123,12 @@ static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32
   if (!ctx || !ctx->V || !points || n == 0) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  float* d_pts = nullptr; unsigned long long* d_keys = nullptr; uint32_t* d_v = nullptr; int32_t* d_f = nullptr; float* d_b = nullptr;
-  CK(dalloc(&d_keys, (size_t)n));
+  DeviceBuffer<float> d_pts, d_b; DeviceBuffer<unsigned long long> d_keys; DeviceBuffer<uint32_t> d_v; DeviceBuffer<int32_t> d_f;
+  CK(d_keys.reserve((size_t)n));
   CK(cudaMemsetAsync(d_keys, 0xff, sizeof(unsigned long long) * (size_t)n, ctx->stream));
   const float* pts = points;
   if (!dev) {
-    CK(dalloc(&d_pts, 3 * (size_t)n)); CK(dalloc(&d_v, (size_t)n)); CK(dalloc(&d_f, (size_t)n)); CK(dalloc(&d_b, 3 * (size_t)n));
+    CK(d_pts.reserve(3 * (size_t)n)); CK(d_v.reserve((size_t)n)); CK(d_f.reserve((size_t)n)); CK(d_b.reserve(3 * (size_t)n));
     CK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
     pts = d_pts;
   }
@@ -1140,9 +1148,7 @@ static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32
     if (out_bary) CK(cudaMemcpyAsync(out_bary, d_b, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   }
   CK(cudaStreamSynchronize(ctx->stream));
-  dfree(d_pts); dfree(d_keys); dfree(d_v); dfree(d_f); dfree(d_b);
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = launches + 1; ctx->stats.settled = n;
+  simple_stats(ctx, launches + 1, n);
   return MNB_OK;
 }
 
@@ -1165,7 +1171,7 @@ int32_t mnb_debug_get_label_sides(mnb_ctx* ctx, uint32_t* root, uint32_t* ext, u
   if (!ctx || !ctx->ws.state) return MNB_E_ARG;
   CK(cudaMemcpy(root, ctx->ws.root, sizeof(uint32_t) * (size_t)ctx->V, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(ext, ctx->ws.ext, sizeof(uint32_t) * (size_t)ctx->V, cudaMemcpyDeviceToHost));
-  if (n_pool) CK(cudaMemcpy(pool, ctx->ws.pool, sizeof(uint32_t) * (size_t)std::min<uint32_t>(n_pool, ctx->ws.pool_cap), cudaMemcpyDeviceToHost));
+  if (n_pool) CK(cudaMemcpy(pool, ctx->ws.pool, sizeof(uint32_t) * (size_t)std::min<uint32_t>(n_pool, ws_pool_cap(ctx->V)), cudaMemcpyDeviceToHost));
   return MNB_OK;
 }
 
@@ -1182,17 +1188,17 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
   if ((rc = ensure_workspace(ctx, 1)) != MNB_OK) return rc;
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   if ((rc = ensure_out(ctx, (size_t)ctx->V, false)) != MNB_OK) return rc;
-  if (!ctx->d_out_cost) CK(dalloc(&ctx->d_out_cost, (size_t)ctx->V));
-  if (n > ctx->lethal_cap) { dfree(ctx->d_lethals); CK(dalloc(&ctx->d_lethals, (size_t)n)); ctx->lethal_cap = n; }
+  CK(ctx->d_out_cost.reserve(ctx->V));
+  CK(ctx->d_lethals.reserve(n));
   if (n) CK(cudaMemcpyAsync(ctx->d_lethals, lethals, sizeof(uint32_t) * n, in_kind(ctx), ctx->stream));
   if (invalid) {
-    if (!ctx->d_infl_invalid) CK(dalloc(&ctx->d_infl_invalid, (size_t)ctx->V));
+    CK(ctx->d_infl_invalid.reserve(ctx->V));
     CK(cudaMemcpyAsync(ctx->d_infl_invalid, invalid, (size_t)ctx->V, in_kind(ctx), ctx->stream));
   }
   CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
   InflateKernelArgs a{};
   a.V = ctx->V; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx; a.cor_wd = ctx->d_cor_wd; a.cor_eid = ctx->d_cor_eid;
-  a.invalid = invalid ? ctx->d_infl_invalid : nullptr; a.ws = ctx->ws; a.lethals = ctx->d_lethals; a.n_lethals = n;
+  a.invalid = invalid ? ctx->d_infl_invalid.p : nullptr; a.ws = wave_workspace(ctx); a.lethals = ctx->d_lethals; a.n_lethals = n;
   a.max_distance = (float)params->inflation_radius;      // double -> `const float&` parameter (inflation_layer.cpp:240,450)
   a.params.inscribed_radius = params->inscribed_radius; a.params.inflation_radius = params->inflation_radius;
   a.params.lethal_value = params->lethal_value; a.params.inscribed_value = params->inscribed_value;
@@ -1218,8 +1224,8 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
   const size_t V = ctx->V;
   if (want_update) {
     const uint32_t n_tiles = (uint32_t)((V + US_TILE - 1) / US_TILE);
-    if (!ctx->d_changed) { CK(dalloc(&ctx->d_changed, V)); CK(dalloc(&ctx->d_tile_count, (size_t)n_tiles)); CK(dalloc(&ctx->d_total, (size_t)1)); }
-    const float* old = ctx->prev_risk_valid ? ctx->d_prev_risk : nullptr;
+    CK(ctx->d_changed.reserve(V)); CK(ctx->d_tile_count.reserve(n_tiles)); CK(ctx->d_total.reserve(1));
+    const float* old = ctx->prev_risk_valid ? ctx->d_prev_risk.p : nullptr;
     uint32_t* d_out = (dev && out_changed) ? out_changed : ctx->d_changed;
     MNB_LAUNCH(k_update_set_count, n_tiles, 256, 0, ctx->stream, (const float*)a.out_cost, old, ctx->V, ctx->d_tile_count);
     MNB_LAUNCH(k_update_set_scan, 1, 1024, 0, ctx->stream, ctx->d_tile_count, n_tiles, ctx->d_total);
@@ -1232,12 +1238,12 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
     if (!dev && out_changed && total) CK(cudaMemcpyAsync(out_changed, d_out, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
     ctx->stats.kernel_launches += 3;
   }
-  if (!ctx->d_prev_risk) CK(dalloc(&ctx->d_prev_risk, V));
+  CK(ctx->d_prev_risk.reserve(V));
   CK(cudaMemcpyAsync(ctx->d_prev_risk, a.out_cost, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->prev_risk_valid = true;
   ctx->infl_labels_valid = true; ctx->infl_had_invalid = invalid != nullptr; ctx->infl_params = *params; ctx->infl_field_valid = false; ctx->infl_rounds = ctx->stats.rounds;
-  if (!ctx->d_infl_dist) CK(dalloc(&ctx->d_infl_dist, V));
+  CK(ctx->d_infl_dist.reserve(V));
   CK(cudaMemcpyAsync(ctx->d_infl_dist, a.out_dist, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));   // distances_
   CK(cudaStreamSynchronize(ctx->stream));
   return MNB_OK;
@@ -1277,14 +1283,13 @@ static int32_t impl_update_vertex_costs(mnb_ctx* ctx, uint32_t n_changed, const 
   const uint32_t* d_ids = changed; const float* d_costs = costs;
   if (!dev) {
     const size_t nc = costs_indexed_by_vertex ? (size_t)ctx->V : (size_t)n_changed;
-    if (n_changed > ctx->upd_cap) { dfree(ctx->d_upd_ids); ctx->upd_cap = 0; CK(dalloc(&ctx->d_upd_ids, (size_t)n_changed)); ctx->upd_cap = n_changed; }
-    if (nc > ctx->upd_cost_cap) { dfree(ctx->d_upd_costs); ctx->upd_cost_cap = 0; CK(dalloc(&ctx->d_upd_costs, nc)); ctx->upd_cost_cap = nc; }
+    CK(ctx->d_upd_ids.reserve(n_changed)); CK(ctx->d_upd_costs.reserve(nc));
     CK(cudaMemcpyAsync(ctx->d_upd_ids, changed, sizeof(uint32_t) * (size_t)n_changed, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_upd_costs, costs, sizeof(float) * nc, cudaMemcpyHostToDevice, ctx->stream));
     d_ids = ctx->d_upd_ids; d_costs = ctx->d_upd_costs;
   }
   if (!ctx->d_upd_stamp || ctx->upd_call == 0xffffffffu) {
-    if (!ctx->d_upd_stamp) CK(dalloc(&ctx->d_upd_stamp, (size_t)ctx->V));
+    CK(ctx->d_upd_stamp.reserve(ctx->V));
     CK(cudaMemsetAsync(ctx->d_upd_stamp, 0, sizeof(uint32_t) * (size_t)ctx->V, ctx->stream));
     ctx->upd_call = 0;
   }
@@ -1302,7 +1307,7 @@ static int32_t impl_update_vertex_costs(mnb_ctx* ctx, uint32_t n_changed, const 
     r.changed = d_ids; r.n = n_changed; r.V = ctx->V; r.faces = ctx->d_faces; r.cor_ptr = ctx->d_cor_ptr; r.cor_idx = ctx->d_cor_idx;
     r.cor_eid = ctx->d_cor_eid; r.face_cor = ctx->d_face_cor; r.adj_ptr = ctx->d_adj_ptr; r.adj_nbr = ctx->d_adj_nbr; r.adj_eid = ctx->d_adj_eid; r.w = ctx->d_edge_w;
     r.cor_w = ctx->d_cor_w; r.ell_w = ctx->d_ell_w; r.ell_geo = ctx->d_ell_geo;
-    r.adj_nw = ctx->adj_dirty ? nullptr : ctx->d_adj_nw; r.ell_adj = ctx->adj_dirty ? nullptr : ctx->d_ell_adj;   // stale tables are rebuilt whole anyway
+    r.adj_nw = ctx->adj_dirty ? nullptr : ctx->d_adj_nw.p; r.ell_adj = ctx->adj_dirty ? nullptr : ctx->d_ell_adj.p;   // stale tables are rebuilt whole anyway
     r.stamp = ctx->d_upd_stamp; r.call = ctx->upd_call;
     MNB_LAUNCH(k_refresh_weight_tables, blocks, 256, 0, ctx->stream, r);
     launches = 3;
@@ -1310,8 +1315,7 @@ static int32_t impl_update_vertex_costs(mnb_ctx* ctx, uint32_t n_changed, const 
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = launches; ctx->stats.settled = n_changed;
+  simple_stats(ctx, launches, n_changed);
   return MNB_OK;
 }
 
@@ -1330,44 +1334,36 @@ static int32_t combination_update(mnb_ctx* ctx, uint32_t n_layers, const float* 
   CombineArgs a{};
   a.n_layers = n_layers; a.n = n_changed; a.V = ctx->V; a.average = weights ? 1 : 0;
   for (uint32_t l = 0; l < n_layers; ++l) a.weight[l] = weights ? weights[l] : 1.0f;
-  std::vector<void*> tmp;                             // host-pointer mode: device copies of the maps
-  auto cleanup = [&]() { for (void* q : tmp) cudaFree(q); };
-  auto up = [&](const void* h, size_t bytes, void** d) -> cudaError_t {
-    cudaError_t e = cudaMalloc(d, bytes ? bytes : 1); if (e != cudaSuccess) return e;
-    tmp.push_back(*d);
-    return cudaMemcpyAsync(*d, h, bytes, cudaMemcpyHostToDevice, ctx->stream);
+  // host-pointer mode: device copies of the maps, for this call
+  DeviceBuffer<float> d_costs[COMB_MAX_LAYERS], d_io; DeviceBuffer<uint8_t> d_lethal[COMB_MAX_LAYERS], d_il; DeviceBuffer<uint32_t> d_ids;
+  auto up = [&](auto& buf, const auto* h, size_t n) -> cudaError_t {
+    const cudaError_t e = buf.reserve(n);
+    return e != cudaSuccess ? e : cudaMemcpyAsync(buf, h, sizeof(*h) * n, cudaMemcpyHostToDevice, ctx->stream);
   };
-  cudaError_t e = cudaSuccess;
-  for (uint32_t l = 0; l < n_layers && e == cudaSuccess; ++l) {
+  for (uint32_t l = 0; l < n_layers; ++l) {
     a.def[l] = defaults[l];
     if (dev) { a.costs[l] = layer_costs[l]; a.lethal[l] = layer_lethal ? layer_lethal[l] : nullptr; continue; }
-    void* d = nullptr;
-    e = up(layer_costs[l], sizeof(float) * V, &d); a.costs[l] = (const float*)d;
-    if (e == cudaSuccess && layer_lethal && layer_lethal[l]) { e = up(layer_lethal[l], V, &d); a.lethal[l] = (const uint8_t*)d; }
+    CK(up(d_costs[l], layer_costs[l], V)); a.costs[l] = d_costs[l];
+    if (layer_lethal && layer_lethal[l]) { CK(up(d_lethal[l], layer_lethal[l], V)); a.lethal[l] = d_lethal[l]; }
   }
-  void* d_ids = nullptr; void* d_io = nullptr; void* d_il = nullptr;
-  if (!dev && e == cudaSuccess) {
-    e = up(changed, sizeof(uint32_t) * (size_t)n_changed, &d_ids);
-    if (e == cudaSuccess) e = up(io_costs, sizeof(float) * V, &d_io);
-    if (e == cudaSuccess && io_lethal) e = up(io_lethal, V, &d_il);
+  if (!dev) {
+    CK(up(d_ids, changed, n_changed));
+    CK(up(d_io, io_costs, V));
+    if (io_lethal) CK(up(d_il, io_lethal, V));
   }
-  if (e != cudaSuccess) { cleanup(); ctx->err = std::string("mnb_max_combination_update: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
-  a.changed = dev ? changed : (const uint32_t*)d_ids;
-  a.io_costs = dev ? io_costs : (float*)d_io;
-  a.io_lethal = dev ? io_lethal : (uint8_t*)d_il;
-  cudaEventRecord(ctx->ev0, ctx->stream);
+  a.changed = dev ? changed : d_ids;
+  a.io_costs = dev ? io_costs : d_io;
+  a.io_lethal = dev ? io_lethal : d_il;
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
   MNB_LAUNCH(k_max_combination_update, (n_changed + 255) / 256, 256, 0, ctx->stream, a);
-  e = cudaGetLastError();
-  cudaEventRecord(ctx->ev1, ctx->stream);
-  if (e == cudaSuccess && !dev) {
-    e = cudaMemcpyAsync(io_costs, a.io_costs, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess && io_lethal) e = cudaMemcpyAsync(io_lethal, a.io_lethal, V, cudaMemcpyDeviceToHost, ctx->stream);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  if (!dev) {
+    CK(cudaMemcpyAsync(io_costs, a.io_costs, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
+    if (io_lethal) CK(cudaMemcpyAsync(io_lethal, a.io_lethal, V, cudaMemcpyDeviceToHost, ctx->stream));
   }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cleanup();
-  if (e != cudaSuccess) { ctx->err = std::string("mnb_max_combination_update: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = 1; ctx->stats.settled = n_changed;
+  CK(cudaStreamSynchronize(ctx->stream));
+  simple_stats(ctx, 1, n_changed);
   return MNB_OK;
 }
 
@@ -1390,7 +1386,7 @@ static int32_t impl_avg_combination_update(mnb_ctx* ctx, uint32_t n_layers, cons
 int32_t mnb_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* pos, const uint32_t* faces,
                      const uint32_t* edges, uint32_t E) {
   const int32_t rc = guarded(ctx, [&]() { return impl_set_mesh(ctx, V, F, pos, faces, edges, E); });
-  if (rc != MNB_OK && ctx) { free_mesh(ctx); ctx->V = 0; ctx->F = 0; ctx->E = 0; }      // no half-built context
+  if (rc != MNB_OK && ctx) free_mesh(ctx);      // no half-built context (V = F = E = 0)
   return rc;
 }
 int32_t mnb_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face, double cost_limit,

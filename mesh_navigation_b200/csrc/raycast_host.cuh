@@ -1,69 +1,64 @@
 // Host side of the ray caster (kernels_raycast.cuh): BVH build on first use, mnb_cast_rays, mnb_obstacle_update /
-// mnb_obstacle_reset, mnb_normal_clearance.  Included at the end of meshnav.cu (uses mnb_ctx, CK, dalloc, the ordered
-// compaction kernels of kernels_updates.cuh).
+// mnb_obstacle_reset, mnb_normal_clearance.  Included at the end of meshnav.cu (uses mnb_ctx and its RayCasterState, CK,
+// DeviceBuffer, simple_stats, the ordered compaction kernels of kernels_updates.cuh).
 #pragma once
 #ifndef MNB_EMU_ACTIVE
 #include <cub/device/device_radix_sort.cuh>
 #endif
 
-static void free_raycaster(mnb_ctx* c) {
-  RayBvh& t = c->bvh;
-  dfree(t.lo); dfree(t.hi); dfree(t.parent); dfree(t.visits); dfree(t.keys); dfree(t.order); dfree(t.keys_tmp); dfree(t.order_tmp);
-  dfree(t.scene);
-  t = RayBvh{};
-  c->bvh_valid = false;
-  dfree(c->d_obst_now); dfree(c->d_obst_mask); dfree(c->d_obst_member); dfree(c->d_obst_member_chg); dfree(c->d_obst_list);
-  dfree(c->d_ray_overflow); dfree(c->d_ray_in); c->ray_in_cap = 0; dfree(c->d_ray_out); c->ray_out_cap = 0;
+// the kernels' view of the tree: a plain struct of raw pointers, passed by value.  The Morton keys exist during the build only.
+static RayBvh ray_bvh(const mnb_ctx* ctx, unsigned long long* keys = nullptr) {
+  RayBvh t{};
+  t.n = ctx->F; t.eps = ctx->bvh_eps; t.lo = ctx->bvh_lo; t.hi = ctx->bvh_hi; t.parent = ctx->bvh_parent; t.visits = ctx->bvh_visits;
+  t.keys = keys; t.order = ctx->bvh_order; t.scene = ctx->bvh_scene;
+  return t;
 }
 
-// Morton order of the faces: radix sort of (key, face id) pairs on the device (stable: equal keys keep ascending face ids)
-static int32_t sort_morton(mnb_ctx* ctx, RayBvh& t) {
+// Morton order of the faces: radix sort of (key, face id) pairs on the device (stable: equal keys keep ascending face ids).
+// The sorted pairs end up in keys / order.
+static int32_t sort_morton(mnb_ctx* ctx, uint32_t n, DeviceBuffer<unsigned long long>& keys, DeviceBuffer<unsigned long long>& keys_tmp,
+                           DeviceBuffer<uint32_t>& order, DeviceBuffer<uint32_t>& order_tmp) {
 #ifdef MNB_EMU_ACTIVE
-  std::vector<uint32_t> idx(t.n);
-  for (uint32_t i = 0; i < t.n; ++i) idx[i] = i;
-  std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return t.keys[a] < t.keys[b]; });
-  for (uint32_t i = 0; i < t.n; ++i) { t.keys_tmp[i] = t.keys[idx[i]]; t.order_tmp[i] = t.order[idx[i]]; }
-  std::swap(t.keys, t.keys_tmp); std::swap(t.order, t.order_tmp);
+  std::vector<uint32_t> idx(n);
+  for (uint32_t i = 0; i < n; ++i) idx[i] = i;
+  std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return keys[a] < keys[b]; });
+  for (uint32_t i = 0; i < n; ++i) { keys_tmp[i] = keys[idx[i]]; order_tmp[i] = order[idx[i]]; }
 #else
   size_t bytes = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, t.keys, t.keys_tmp, t.order, t.order_tmp, (int)t.n, 0, 63, ctx->stream));
-  void* tmp = nullptr;
-  CK(cudaMalloc(&tmp, bytes ? bytes : 1));
-  const cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, bytes, t.keys, t.keys_tmp, t.order, t.order_tmp, (int)t.n, 0, 63, ctx->stream);
-  const cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
-  cudaFree(tmp);
-  CK(e); CK(e2);
-  std::swap(t.keys, t.keys_tmp); std::swap(t.order, t.order_tmp);
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys.p, keys_tmp.p, order.p, order_tmp.p, (int)n, 0, 63, ctx->stream));
+  DeviceBuffer<unsigned char> tmp;
+  CK(tmp.reserve(bytes ? bytes : 1));
+  CK(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys.p, keys_tmp.p, order.p, order_tmp.p, (int)n, 0, 63, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
 #endif
+  std::swap(keys, keys_tmp); std::swap(order, order_tmp);
   return MNB_OK;
 }
 
-static int32_t ensure_raycaster(mnb_ctx* ctx) {
-  if (ctx->bvh_valid) return MNB_OK;
-  if (!ctx->V || !ctx->F) { ctx->err = "ray casting needs a mesh with faces"; return MNB_E_STATE; }
-  RayBvh& t = ctx->bvh;
+static int32_t build_raycaster(mnb_ctx* ctx) {
   const uint32_t n = ctx->F;
   const size_t nodes = 2 * (size_t)n - 1;
-  t.n = n;
-  CK(dalloc(&t.lo, nodes)); CK(dalloc(&t.hi, nodes)); CK(dalloc(&t.parent, nodes)); CK(dalloc(&t.visits, (size_t)n));
-  CK(dalloc(&t.keys, (size_t)n)); CK(dalloc(&t.order, (size_t)n)); CK(dalloc(&t.keys_tmp, (size_t)n)); CK(dalloc(&t.order_tmp, (size_t)n));
-  CK(dalloc(&t.scene, (size_t)8));
+  DeviceBuffer<unsigned long long> keys, keys_tmp; DeviceBuffer<uint32_t> order_tmp;      // of the build: only the tree and the face order are kept
+  CK(ctx->bvh_lo.reserve(nodes)); CK(ctx->bvh_hi.reserve(nodes)); CK(ctx->bvh_parent.reserve(nodes)); CK(ctx->bvh_visits.reserve(n));
+  CK(keys.reserve(n)); CK(ctx->bvh_order.reserve(n)); CK(keys_tmp.reserve(n)); CK(order_tmp.reserve(n));
+  CK(ctx->bvh_scene.reserve(8));
   const unsigned int scene0[8] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u, 0u};
-  CK(cudaMemcpyAsync(t.scene, scene0, sizeof(scene0), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemsetAsync(t.visits, 0, sizeof(unsigned int) * (size_t)n, ctx->stream));
-  CK(cudaMemsetAsync(t.parent, 0xff, sizeof(uint32_t) * nodes, ctx->stream));
-  MNB_LAUNCH(k_bvh_scene, 2 * ctx->sm_count, 256, 0, ctx->stream, (const float*)ctx->d_pos, ctx->V, t.scene);
+  CK(cudaMemcpyAsync(ctx->bvh_scene, scene0, sizeof(scene0), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(ctx->bvh_visits, 0, sizeof(unsigned int) * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(ctx->bvh_parent, 0xff, sizeof(uint32_t) * nodes, ctx->stream));
+  MNB_LAUNCH(k_bvh_scene, 2 * ctx->sm_count, 256, 0, ctx->stream, (const float*)ctx->d_pos, ctx->V, ctx->bvh_scene);
   MNB_LAUNCH(k_bvh_morton, (n + 255) / 256, 256, 0, ctx->stream, (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces, n,
-             (const unsigned int*)t.scene, t.keys, t.order);
+             (const unsigned int*)ctx->bvh_scene, keys, ctx->bvh_order);
   CK(cudaGetLastError());
   unsigned int scene[8];
-  CK(cudaMemcpyAsync(scene, t.scene, sizeof(scene), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(scene, ctx->bvh_scene, sizeof(scene), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   float mx; std::memcpy(&mx, &scene[6], 4);
-  t.eps = 1e-5f * mx;
-  if (!(t.eps > 0.0f)) t.eps = 1e-30f;
-  int32_t rc = sort_morton(ctx, t);
+  ctx->bvh_eps = 1e-5f * mx;
+  if (!(ctx->bvh_eps > 0.0f)) ctx->bvh_eps = 1e-30f;
+  int32_t rc = sort_morton(ctx, n, keys, keys_tmp, ctx->bvh_order, order_tmp);
   if (rc != MNB_OK) return rc;
+  const RayBvh t = ray_bvh(ctx, keys);
   MNB_LAUNCH(k_bvh_leaves, (n + 255) / 256, 256, 0, ctx->stream, (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces, t);
   if (n > 1) {
     MNB_LAUNCH(k_bvh_tree, (n - 1 + 255) / 256, 256, 0, ctx->stream, t);
@@ -71,10 +66,17 @@ static int32_t ensure_raycaster(mnb_ctx* ctx) {
   }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(ctx->stream));
-  dfree(t.keys_tmp); dfree(t.order_tmp); dfree(t.keys);          // only the tree and the face order are kept
-  if (!ctx->d_ray_overflow) CK(dalloc(&ctx->d_ray_overflow, (size_t)1));
+  CK(ctx->d_ray_overflow.reserve(1));
   ctx->bvh_valid = true;
   return MNB_OK;
+}
+
+static int32_t ensure_raycaster(mnb_ctx* ctx) {
+  if (ctx->bvh_valid) return MNB_OK;
+  if (!ctx->V || !ctx->F) { ctx->err = "ray casting needs a mesh with faces"; return MNB_E_STATE; }
+  const int32_t rc = build_raycaster(ctx);
+  if (rc != MNB_OK) free_raycaster(ctx);       // no partial tree for the next call to allocate over
+  return rc;
 }
 
 static int32_t check_ray_overflow(mnb_ctx* ctx) {
@@ -87,8 +89,7 @@ static int32_t check_ray_overflow(mnb_ctx* ctx) {
 
 // staging of host-pointer inputs / outputs of the ray calls (floats)
 static int32_t ensure_ray_io(mnb_ctx* ctx, size_t n_in, size_t n_out) {
-  if (n_in > ctx->ray_in_cap) { dfree(ctx->d_ray_in); CK(dalloc(&ctx->d_ray_in, n_in)); ctx->ray_in_cap = n_in; }
-  if (n_out > ctx->ray_out_cap) { dfree(ctx->d_ray_out); CK(dalloc(&ctx->d_ray_out, n_out)); ctx->ray_out_cap = n_out; }
+  CK(ctx->d_ray_in.reserve(n_in)); CK(ctx->d_ray_out.reserve(n_out));
   return MNB_OK;
 }
 
@@ -110,14 +111,14 @@ static int32_t impl_cast_rays(mnb_ctx* ctx, uint32_t n, const float* origins, co
     CK(cudaMemcpyAsync(ctx->d_ray_in, origins, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_ray_in + 3 * (size_t)n, dirs, sizeof(float) * nd, cudaMemcpyHostToDevice, ctx->stream));
     d_o = ctx->d_ray_in; d_d = ctx->d_ray_in + 3 * (size_t)n;
-    d_dist = out_dist ? ctx->d_ray_out : nullptr;
+    d_dist = out_dist ? ctx->d_ray_out.p : nullptr;
     d_face = out_face ? (uint32_t*)(ctx->d_ray_out + n) : nullptr;
     d_point = out_point ? ctx->d_ray_out + 2 * (size_t)n : nullptr;
     d_hit = out_hit ? (uint8_t*)(ctx->d_ray_out + 5 * (size_t)n) : nullptr;
   }
   CK(cudaMemsetAsync(ctx->d_ray_overflow, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  MNB_LAUNCH(k_cast_rays, (n + 127) / 128, 128, 0, ctx->stream, ctx->bvh, (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces, n,
+  MNB_LAUNCH(k_cast_rays, (n + 127) / 128, 128, 0, ctx->stream, ray_bvh(ctx), (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces, n,
              d_o, d_d, dir_stride, d_hit, d_dist, d_face, d_point, ctx->d_ray_overflow);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
@@ -128,8 +129,7 @@ static int32_t impl_cast_rays(mnb_ctx* ctx, uint32_t n, const float* origins, co
     if (out_hit) CK(cudaMemcpyAsync(out_hit, d_hit, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if ((rc = check_ray_overflow(ctx)) != MNB_OK) return rc;
-  float ms = 0; CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-  ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = 1; ctx->stats.settled = n;
+  simple_stats(ctx, 1, n);
   return MNB_OK;
 }
 
@@ -152,11 +152,11 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   const uint32_t n_tiles = (uint32_t)((V + US_TILE - 1) / US_TILE);
   if (!ctx->d_obst_mask) {
-    CK(dalloc(&ctx->d_obst_now, V)); CK(dalloc(&ctx->d_obst_mask, V)); CK(dalloc(&ctx->d_obst_member, V));
-    CK(dalloc(&ctx->d_obst_member_chg, V)); CK(dalloc(&ctx->d_obst_list, 2 * V));
+    CK(ctx->d_obst_now.reserve(V)); CK(ctx->d_obst_mask.reserve(V)); CK(ctx->d_obst_member.reserve(V));
+    CK(ctx->d_obst_member_chg.reserve(V)); CK(ctx->d_obst_list.reserve(2 * V));
     CK(cudaMemsetAsync(ctx->d_obst_mask, 0, V, ctx->stream));
   }
-  if (!ctx->d_changed) { CK(dalloc(&ctx->d_changed, V)); CK(dalloc(&ctx->d_tile_count, (size_t)n_tiles)); CK(dalloc(&ctx->d_total, (size_t)1)); }
+  CK(ctx->d_changed.reserve(V)); CK(ctx->d_tile_count.reserve(n_tiles)); CK(ctx->d_total.reserve(1));
   if ((rc = ensure_ray_io(ctx, dev ? 0 : 3 * (size_t)n_points, (!dev && out_costs) ? V : 0)) != MNB_OK) return rc;
   const float* d_pts = points;
   if (!dev && n_points) {
@@ -174,7 +174,7 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
   CK(cudaMemsetAsync(ctx->d_ray_overflow, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   if (n_points)
-    MNB_LAUNCH(k_obstacle_rays, (n_points + 127) / 128, 128, 0, ctx->stream, ctx->bvh, (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces,
+    MNB_LAUNCH(k_obstacle_rays, (n_points + 127) / 128, 128, 0, ctx->stream, ray_bvh(ctx), (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces,
                n_points, d_pts, a, ctx->d_obst_now, ctx->d_ray_overflow);
   MNB_LAUNCH(k_obstacle_diff, (unsigned)((V + 255) / 256), 256, 0, ctx->stream, ctx->V, (const uint8_t*)ctx->d_obst_now, ctx->d_obst_mask,
              ctx->d_obst_member, ctx->d_obst_member_chg, d_costs);
@@ -197,8 +197,7 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
     if (out_costs) CK(cudaMemcpyAsync(out_costs, d_costs, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if ((rc = check_ray_overflow(ctx)) != MNB_OK) return rc;
-  float ms = 0; CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = (n_points ? 1 : 0) + 7; ctx->stats.settled = n_points;
+  simple_stats(ctx, (n_points ? 1 : 0) + 7, n_points);
   return MNB_OK;
 }
 
@@ -218,14 +217,13 @@ static int32_t impl_normal_clearance(mnb_ctx* ctx, const float* vertex_normals, 
   float* d_out = dev ? out_clearance : ctx->d_ray_out;
   CK(cudaMemsetAsync(ctx->d_ray_overflow, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  MNB_LAUNCH(k_normal_clearance, (unsigned)((V + 127) / 128), 128, 0, ctx->stream, ctx->bvh, (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces,
+  MNB_LAUNCH(k_normal_clearance, (unsigned)((V + 127) / 128), 128, 0, ctx->stream, ray_bvh(ctx), (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces,
              ctx->V, d_vn, d_out, ctx->d_ray_overflow);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (!dev) CK(cudaMemcpyAsync(out_clearance, d_out, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
   if ((rc = check_ray_overflow(ctx)) != MNB_OK) return rc;
-  float ms = 0; CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-  ctx->stats = mnb_stats{}; ctx->stats.kernel_ms = ms; ctx->stats.kernel_launches = 1; ctx->stats.settled = ctx->V;
+  simple_stats(ctx, 1, ctx->V);
   return MNB_OK;
 }
 

@@ -576,7 +576,19 @@ static inline cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = new EmuEvent{0.
 static inline cudaError_t cudaEventDestroy(cudaEvent_t e) { delete e; return cudaSuccess; }
 static inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t = nullptr) { e->t_ms = emu::now_ms(); return cudaSuccess; }
 static inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b) { *ms = (float)(b->t_ms - a->t_ms); return cudaSuccess; }
-static inline cudaError_t cudaMalloc(void** p, size_t n) { *p = emu::arena_alloc(n ? n : 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+// MNB_EMU_MALLOC_LIMIT=<bytes> (read at every call): a single request above it fails, as on a device that cannot hold it --
+// tests/test_emu_host_memory.py drives the host code's allocation-failure paths with it
+static inline cudaError_t cudaMalloc(void** p, size_t n) {
+  const char* limit = getenv("MNB_EMU_MALLOC_LIMIT");
+  *p = (limit && n > strtoull(limit, nullptr, 10)) ? nullptr : emu::arena_alloc(n ? n : 1);
+  return *p ? cudaSuccess : cudaErrorMemoryAllocation;
+}
+// bytes allocated from the arena and not freed (whole 4096-byte pages per allocation): the leak probe of the same tests
+extern "C" __attribute__((used, visibility("default"))) inline size_t mnb_emu_allocated_bytes() {
+  size_t sum = 0;
+  if (emu::g_sizes) for (const auto& kv : *emu::g_sizes) sum += kv.second;
+  return sum;
+}
 static inline cudaError_t cudaFree(void* p) { emu::arena_free(p); return cudaSuccess; }
 static inline cudaError_t cudaHostAlloc(void** p, size_t n, unsigned) { return cudaMalloc(p, n); }
 static inline cudaError_t cudaFreeHost(void* p) { return cudaFree(p); }
