@@ -164,6 +164,26 @@ int32_t mnb_cvp_matrix(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n
                        uint32_t m, const uint32_t* target_vertices /* m, host */, double cost_limit,
                        float* out /* [n][m] */);
 
+/* Dijkstra field repair: brings resident distance and predecessor rows up to date after cost updates by re-running only
+ * the region the change can reach.  On entry row k of io_dist / io_pred ([n][V] row-major) is the field of
+ * mnb_dijkstra_batch(seed_vertices[k], cost_limit) -- or, the same thing, of a full-field mnb_dijkstra (robot vertex
+ * -1) -- computed on the costs installed before one or more mnb_update_vertex_costs calls, and changed[n_changed] holds
+ * the union of those calls' changed sets (any order, duplicates and vertices whose cost did not change allowed).  On
+ * return row k is bit-identical to mnb_dijkstra_batch on the current costs, predecessors included.
+ * The caller is responsible for the changed set: a vertex left out of it leaves its region stale.  mnb_set_costs or
+ * mnb_compute_edge_weights between the rows and the repair invalidate the rows unless every vertex is passed as changed.
+ * Work: the vertices whose predecessor chain runs through a changed vertex are reset and re-reached, the rest keep their
+ * labels unless the change lowers them.  mnb_get_stats reports rounds, recomputes and settled vertices summed over the
+ * waves, as for mnb_dijkstra_batch.  seed_vertices and changed are host pointers; the rows follow mnb_set_pointer_mode:
+ * device rows are repaired in place, host rows are uploaded and downloaded.  n_changed == 0 returns MNB_SUCCESS and
+ * leaves the rows untouched.  Errors, with nothing written: MNB_E_ARG for n == 0, a NULL array or a changed vertex >= V;
+ * MNB_E_STATE without costs; MNB_INVALID_START for a seed >= V.  MNB_CANCELED after mnb_cancel: the rows are then not
+ * valid, and the caller recomputes them (mnb_dijkstra_batch).  Runs in mnb_dijkstra_batch's workspace, under the same
+ * memory cap: the results of the last mnb_cvp and of the last inflation stay available. */
+int32_t mnb_dijkstra_batch_repair(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices /* n, host */, double cost_limit,
+                                  uint32_t n_changed, const uint32_t* changed /* n_changed, host */,
+                                  float* io_dist /* [n][V] */, uint32_t* io_pred /* [n][V] */);
+
 /* ---- InflationLayer::waveCostInflation (inflation_layer.cpp:341-491) -----
  * lethals[n] (any order, duplicates allowed).  Uses edge_distances (:383), not edge_weights.
  * out_dist[V]: distances_ (+inf = not in the sparse map); out_cost[V]: riskiness_ =

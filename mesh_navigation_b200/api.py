@@ -254,6 +254,14 @@ class MeshMap:
         tv = np.ascontiguousarray(target_vertices, dtype=np.uint32).reshape(-1)
         return self._check(self.L.mnb_dijkstra_matrix(self._ctx, sv.size, _p(sv), tv.size, _p(tv), float(cost_limit), _p(d_out)))
 
+    def dijkstra_batch_repair_dev(self, seed_vertices, changed, cost_limit, d_dist: int, d_pred: int) -> int:
+        """mnb_dijkstra_batch_repair on device rows ([n,V] dist and pred, repaired in place); seeds and the changed
+        vertices are host values"""
+        sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32).reshape(-1)
+        ch = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        return self._check(self.L.mnb_dijkstra_batch_repair(self._ctx, sv.size, _p(sv), float(cost_limit), ch.size, _p(ch),
+                                                            _p(d_dist), _p(d_pred)))
+
     def cvp_matrix_dev(self, seed_faces, seed_pos, target_vertices, cost_limit, d_out: int) -> int:
         """mnb_cvp_matrix with a device output ([n,m]); seeds and targets are host values"""
         sf = np.ascontiguousarray(seed_faces, dtype=np.uint32).reshape(-1)
@@ -297,6 +305,20 @@ class DijkstraMeshPlanner:
         cost = np.empty((sv.size, tv.size), dtype=np.float32)
         rc = m._check(m.L.mnb_dijkstra_matrix(m._ctx, sv.size, _p(sv), tv.size, _p(tv), float(self.cost_limit), _p(cost)))
         return dict(outcome=rc, cost=cost, **m.stats())
+
+    def dijkstraBatchRepair(self, seed_vertices, changed, dist, pred):
+        """brings the rows of dijkstraBatch(seed_vertices) (dist f32 [n,V], pred u32 [n,V], updated in place) up to date
+        after layerChanged calls whose changed vertices are `changed` (their union); afterwards the rows are bit-identical
+        to a fresh dijkstraBatch on the current costs.  Only the region the change can reach is re-run."""
+        m = self.map
+        sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32).reshape(-1)
+        ch = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        for a, t in ((dist, np.float32), (pred, np.uint32)):
+            if a.dtype != t or not a.flags.c_contiguous or a.shape != (sv.size, m.V):
+                raise ValueError(f"rows must be C-contiguous {np.dtype(t).name} arrays of shape ({sv.size}, {m.V})")
+        rc = m._check(m.L.mnb_dijkstra_batch_repair(m._ctx, sv.size, _p(sv), float(self.cost_limit), ch.size, _p(ch),
+                                                    _p(dist), _p(pred)))
+        return dict(outcome=rc, dist=dist, pred=pred, **m.stats())
 
     def computeVectorMap(self, pred):
         return self.map.vectorMap(pred)

@@ -69,6 +69,9 @@ __device__ __forceinline__ uint4 state_inf() { return make_uint4(INF_BITS, INF_B
 // Comparison of pop times.  `pool` is the level pool of the wavefront (only dereferenced when two times tie through a
 // level whose id or key lives there -- never on the hot path).
 struct TimeAlg {
+  // a problem that repairs a finished field (DijkstraRepairProblem) activates on a change of label and logs the vertices
+  // it marks (run_band_rounds); every other problem is a fresh wave
+  static constexpr bool REPAIR = false;
   const uint32_t* pool = nullptr;
   __device__ __forceinline__ uint32_t id2_of(const EvTime& t) const {      // id of level 2 (level 2 must exist)
     return t.a3 == 0.0f ? t.self : ((t.ext & EXT_POOL) ? __ldcg(&pool[(t.ext & ~EXT_POOL) + 1]) : t.ext);
@@ -491,12 +494,17 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
       }
       if (!nf) my_lo = fminf(my_lo, ntau);      // smallest pop time still in flight: the band follows it
       stage_push(st, c, list_n, &ctl->count[next]);
-      // a vertex that holds a finite label pulls its neighbours into the candidate set (once)
-      if (__float_as_uint(nd) != INF_BITS && __ldcg(&mark[c]) == MARK_CAND) {
+      // a vertex that holds a finite label pulls its neighbours into the candidate set (once).  In a repair most
+      // candidates hold finite labels from the start, so the pull waits for the first change of the label -- in a fresh
+      // wave the same moment as the first finite label -- and every vertex it marks is logged for the reset of the marks.
+      const bool pull = P::REPAIR ? changed : __float_as_uint(nd) != INF_BITS;
+      if (pull && __ldcg(&mark[c]) == MARK_CAND) {
         mark[c] = MARK_CAND_ACT;
         prob.activate(c, [&](uint32_t x) {
-          if (__ldcg(&mark[x]) == MARK_NONE && prob.eligible(x) && atomicCAS(&mark[x], MARK_NONE, MARK_CAND) == MARK_NONE)
+          if (__ldcg(&mark[x]) == MARK_NONE && prob.eligible(x) && atomicCAS(&mark[x], MARK_NONE, MARK_CAND) == MARK_NONE) {
+            if constexpr (P::REPAIR) prob.log_mark(x);
             stage_push(st, x, list_n, &ctl->count[next]);
+          }
         });
       }
     };

@@ -601,6 +601,147 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijk
   }
 }
 
+// Field repair (mnb_dijkstra_batch_repair): row q of out_dist / out_pred holds the field of seeds[q] on the costs before
+// an update of the vertices in chg, and is brought up to date in place.
+struct RepairSet {
+  const uint32_t* list;         // [n] device: the distinct changed vertices
+  const uint32_t* bits;         // [V/32 + 1] device: their bitmap
+  uint32_t n;
+  unsigned int* log_n;          // [groups] device: length of the group's log of marked vertices (zero between waves)
+};
+struct DijkstraRepairArgs : DijkstraBatchArgs {
+  RepairSet chg;
+};
+
+// The final field is a function of the weights, the gates and the seed alone, so the repair re-runs the wave from the
+// old labels that are still realizable (DESIGN §4):
+//  1. D = the changed vertices and their descendants in the old predecessor tree, found level by level (x is a child of u
+//     iff pred[x] == u), without the seed.  D gets +inf and pred = self.  Every other label is the float sum of a path
+//     whose weights and gates did not change: an upper bound of the new distance.
+//  2. The first candidates are the changed vertices, their neighbours and the vertices of D next to a finite label that
+//     expands.  They are evaluated once without the band filter, so a candidate whose source lies beyond the band holds a
+//     finite label from the start; the band starts at the smallest label of the list.  A candidate that changes pulls its
+//     neighbours in, as in the round loop.
+//  3. The round loop of the batch (run_band_rounds with DijkstraRepairProblem): labels never rise, and a candidate
+//     activates its ring when its label first changes.
+//  4. The marks the wave set are reset through its log: the mark array is clean between waves without a V-sized pass.
+// The label workspace is not used by the repair (the rows are the labels); its first V words of the group hold the log.
+template <int CS>
+__global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijkstra_batch_repair(const DijkstraRepairArgs a) {
+  __shared__ Stage st;
+  __shared__ float s_lo;
+  uint32_t g, gthreads, gtid;
+  group_coords<CS>(g, gthreads, gtid);
+  const uint32_t V = a.V;
+  uint32_t* mark = a.ws.mark + (size_t)g * V;
+  uint32_t* list0 = a.ws.list0 + (size_t)g * V;
+  uint32_t* list1 = a.ws.list1 + (size_t)g * V;
+  GroupCtl* ctl = a.ws.ctl + g;
+  const volatile int* cancel = a.cancel_flag;
+  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  __syncthreads();
+  DijkstraRepairProblem prob;
+  prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
+  prob.cost_limit = a.cost_limit; prob.deferred_m = __uint_as_float(INF_BITS);
+  prob.log = reinterpret_cast<uint32_t*>(a.ws.label) + (size_t)g * V; prob.log_n = a.chg.log_n + g;
+  const float INF = __uint_as_float(INF_BITS);
+  auto changed_vertex = [&](uint32_t x) { return (__ldg(&a.chg.bits[x >> 5]) >> (x & 31)) & 1u; };
+  auto expands = [&](uint32_t u) { return (double)__ldg(&a.cost[u]) <= a.cost_limit; };
+  for (;;) {
+    if (gtid == 0) ctl->query = (cancel && *cancel) ? a.n_queries : atomicAdd(a.next_query, 1u);
+    group_sync<CS>();
+    const uint32_t q = __ldcg(&ctl->query);
+    if (q >= a.n_queries) break;
+    float* dist = a.out_dist + (size_t)q * V;
+    uint32_t* pred = a.out_pred + (size_t)q * V;
+    prob.state = dist; prob.pred = pred;
+    const uint32_t s = a.seeds[q];
+    // Before the round loop the rings of the GroupCtl serve as scratch (ctl_reset sets them for the loop): lo[] counts
+    // the levels of D, count[0] the candidates, m_tau[1] holds their smallest label.
+    // 1. D, breadth-first in list1: level 0 the changed vertices (the seed among them only to find its children).  The
+    //    children of level k are counted in lo[k % 3]; thread 0 clears the slot of level k + 1 while level k runs, when
+    //    the last reads of that slot (level k - 2) are behind a barrier.
+    for (uint32_t i = gtid; i < a.chg.n; i += gthreads) list1[i] = a.chg.list[i];
+    if (gtid == 0) { ctl->lo[0] = 0u; ctl->count[0] = 0u; ctl->m_tau[1] = INF_BITS; mark[s] = MARK_FIXED; }
+    group_sync<CS>();
+    uint32_t lb = 0, le = a.chg.n;
+    for (uint32_t lvl = 0; lb < le; ++lvl) {
+      unsigned int* cnt = &ctl->lo[lvl % 3];
+      if (gtid == 0) ctl->lo[(lvl + 1) % 3] = 0u;
+      for (uint32_t i = lb + gtid; i < le; i += gthreads) {
+        const uint32_t u = __ldcg(&list1[i]);
+        prob.activate(u, [&](uint32_t x) {
+          if (__ldcg(&pred[x]) == u && !changed_vertex(x)) list1[le + atomicAdd(cnt, 1u)] = x;
+        });
+      }
+      group_sync<CS>();
+      lb = le; le += __ldcg(cnt);
+    }
+    const uint32_t nd = le;
+    for (uint32_t i = gtid; i < nd; i += gthreads) {
+      const uint32_t x = __ldcg(&list1[i]);
+      if (x != s) { dist[x] = INF; pred[x] = x; }
+    }
+    group_sync<CS>();
+    // 2. the first candidates in list0 (marked and logged), then one evaluation without the band filter
+    auto add = [&](uint32_t x) {
+      if (x != s && __ldcg(&mark[x]) == MARK_NONE && prob.eligible(x) && atomicCAS(&mark[x], MARK_NONE, MARK_CAND) == MARK_NONE) {
+        prob.log_mark(x);
+        list0[atomicAdd(&ctl->count[0], 1u)] = x;
+      }
+    };
+    for (uint32_t i = gtid; i < a.chg.n; i += gthreads) {
+      const uint32_t c = a.chg.list[i];
+      add(c);
+      prob.activate(c, add);
+    }
+    for (uint32_t i = gtid; i < nd; i += gthreads) {
+      const uint32_t x = __ldcg(&list1[i]);
+      bool next_to_source = false;
+      prob.activate(x, [&](uint32_t u) { next_to_source |= __float_as_uint(__ldcg(&dist[u])) != INF_BITS && expands(u); });
+      if (next_to_source) add(x);
+    }
+    group_sync<CS>();
+    const uint32_t n_first = __ldcg(&ctl->count[0]);
+    unsigned long long evals = 0;
+    for (uint32_t i = gtid; i < n_first; i += gthreads) {
+      const uint32_t c = __ldcg(&list0[i]);
+      float nv, ntau;
+      evals++;
+      if (prob.recompute(c, INF, INF, 0, prob.load_label(c), nv, ntau)) {
+        mark[c] = MARK_CAND_ACT;
+        prob.activate(c, add);
+      }
+    }
+    if (evals) atomicAdd(&ctl->recomputes, evals);
+    if (threadIdx.x == 0) s_lo = INF;
+    group_sync<CS>();
+    const uint32_t n0 = __ldcg(&ctl->count[0]);
+    float my_lo = INF;
+    for (uint32_t i = gtid; i < n0; i += gthreads) my_lo = fminf(my_lo, __ldcg(&dist[__ldcg(&list0[i])]));
+    const unsigned int wl = __reduce_min_sync(0xffffffffu, __float_as_uint(my_lo));
+    if ((threadIdx.x & 31) == 0 && wl != INF_BITS) atomicMin(reinterpret_cast<unsigned int*>(&s_lo), wl);
+    __syncthreads();
+    if (threadIdx.x == 0 && __float_as_uint(s_lo) != INF_BITS) atomicMin(&ctl->m_tau[1], __float_as_uint(s_lo));
+    group_sync<CS>();
+    // 3. the round loop from the smallest label of the list (ctl->m_tau[1] served as the group's minimum)
+    if (gtid == 0) {
+      const float lo0 = __uint_as_float(__ldcg(&ctl->m_tau[1]));
+      ctl_reset(ctl, n0, lo0);
+    }
+    group_sync<CS>();
+    run_band_rounds<CS>(prob, ctl, list0, list1, mark, st, a.delta, gthreads, gtid, 0, 0xffffffffu, 0xffffffffu, 0xffffffffu,
+                        0.0, a.cancel_flag, 1e-30f, a.max_rounds);
+    group_sync<CS>();
+    // 4. the marks back to MARK_NONE for the next wave
+    const uint32_t nl = __ldcg(prob.log_n);
+    for (uint32_t i = gtid; i < nl; i += gthreads) mark[__ldcg(&prob.log[i])] = MARK_NONE;
+    if (gtid == 0) mark[s] = MARK_NONE;
+    group_sync<CS>();
+    if (gtid == 0) *prob.log_n = 0u;
+  }
+}
+
 // Single Dijkstra plan on the whole GPU: 8 lanes per candidate (one edge each), wide band + in-round sweeps,
 // same engine instance as k_cvp_grid.
 __global__ void __launch_bounds__(512, 1) k_dijkstra_grid(const DijkstraKernelArgs a) {

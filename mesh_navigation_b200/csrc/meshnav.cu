@@ -93,6 +93,7 @@ struct MeshState : RayCasterState {
   WaveBuffers ws;
   uint32_t dws_groups = 0;       // the batched Dijkstra planner's own workspace (k_dijkstra_batch)
   DijkstraBatchBuffers dws;
+  bool dws_marks_clean = false;  // every mark of dws is MARK_NONE: the repair kernel leaves them so, the batch kernel does not
   DeviceBuffer<uint32_t> d_batch_pred;    // its predecessor rows in host-pointer mode (and mnb_cvp_batch_fields')
   DeviceBuffer<float> d_batch_dir;        // mnb_cvp_batch_fields' direction and cutting-face rows in host-pointer mode
   DeviceBuffer<int32_t> d_batch_cut;
@@ -100,6 +101,8 @@ struct MeshState : RayCasterState {
   DeviceBuffer<float> d_out_dist, d_out_dir, d_out_cost; DeviceBuffer<uint32_t> d_out_pred; DeviceBuffer<int32_t> d_out_cut;
   // target vertices of the cost-matrix calls: the caller's list and the bitmap of the distinct ones (V/32 + 1 words)
   DeviceBuffer<uint32_t> d_targets, d_target_bits;
+  // changed vertices of a field repair: the distinct ones, their bitmap (V/32 + 1 words), the per-group log lengths
+  DeviceBuffer<uint32_t> d_repair_chg, d_repair_bits; DeviceBuffer<unsigned int> d_repair_log_n;
   DeviceBuffer<float> d_face_normals, d_vertex_normals; DeviceBuffer<uint8_t> d_border;
   DeviceBuffer<float> d_layer_costs, d_layer_combined, d_clearance; DeviceBuffer<uint8_t> d_layer_mask;
   DeviceBuffer<float4> d_pos4, d_vn4; DeviceBuffer<uint32_t> d_nbr8;     // packed copies for k_layers<true>
@@ -685,6 +688,33 @@ static int32_t upload_targets(mnb_ctx* ctx, const MatrixRequest& mx, TargetSet& 
   return MNB_OK;
 }
 
+// The changed vertices of a field repair (mnb_dijkstra_batch_repair): host list, any order, duplicates allowed.
+struct RepairRequest { uint32_t n; const uint32_t* changed; };
+
+// MNB_E_ARG if a changed vertex is >= V (nothing written)
+static int32_t check_changed(mnb_ctx* ctx, const RepairRequest* rq) {
+  if (rq) for (uint32_t i = 0; i < rq->n; ++i) if (rq->changed[i] >= ctx->V) return MNB_E_ARG;
+  return MNB_OK;
+}
+
+// Uploads the distinct changed vertices and their bitmap (ctx buffers, freed with the mesh), clears the log lengths of the
+// groups and fills cs.
+static int32_t upload_changed(mnb_ctx* ctx, const RepairRequest& rq, unsigned groups, RepairSet& cs) {
+  const size_t words = ((size_t)ctx->V >> 5) + 1;
+  std::vector<uint32_t> bits(words, 0u), list;     // (a copy from pageable memory has read it when cudaMemcpyAsync returns)
+  list.reserve(rq.n);
+  for (uint32_t i = 0; i < rq.n; ++i) {
+    const uint32_t v = rq.changed[i], bit = 1u << (v & 31);
+    if (!(bits[v >> 5] & bit)) { bits[v >> 5] |= bit; list.push_back(v); }
+  }
+  CK(ctx->d_repair_bits.reserve(words)); CK(ctx->d_repair_chg.reserve(list.size())); CK(ctx->d_repair_log_n.reserve(groups));
+  CK(cudaMemcpyAsync(ctx->d_repair_bits, bits.data(), sizeof(uint32_t) * words, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->d_repair_chg, list.data(), sizeof(uint32_t) * list.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(ctx->d_repair_log_n, 0, sizeof(unsigned int) * groups, ctx->stream));
+  cs.list = ctx->d_repair_chg; cs.bits = ctx->d_repair_bits; cs.n = (uint32_t)list.size(); cs.log_n = ctx->d_repair_log_n;
+  return MNB_OK;
+}
+
 // host-pointer mode: the [n][m] matrix from its device staging (d_out_dist) into the caller's array
 static int32_t copy_matrix_out(mnb_ctx* ctx, uint32_t n, const MatrixRequest* mx) {
   if (mx && ctx->ptr_mode != MNB_PTR_DEVICE)
@@ -913,13 +943,18 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
 // n full-field Dijkstra waves in one launch (k_dijkstra_batch).  The waves run in a workspace of their own, so the
 // results of the last mnb_cvp (predecessors, directions, cutting faces) and the labels of the last inflation stay valid.
 // With mx (mnb_dijkstra_matrix; no row outputs) the waves run the matrix form k_dijkstra_batch<CS, true> into mx->out.
+// With rq (mnb_dijkstra_batch_repair) out_dist / out_pred are the rows to repair (k_dijkstra_batch_repair<CS>), in place
+// in device-pointer mode, through the device staging otherwise.
 static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, float* out_dist,
-                                   uint32_t* out_pred, const MatrixRequest* mx = nullptr) {
+                                   uint32_t* out_pred, const MatrixRequest* mx = nullptr, const RepairRequest* rq = nullptr) {
   if (!ctx || !seed_vertices || (!out_dist && !out_pred && !mx) || !ctx->V || n == 0) return MNB_E_ARG;
+  if (rq && (!out_dist || !out_pred || (rq->n && !rq->changed))) return MNB_E_ARG;
+  int32_t rc;
+  if ((rc = check_changed(ctx, rq)) != MNB_OK) return rc;
   if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
   for (uint32_t i = 0; i < n; ++i) if (seed_vertices[i] >= ctx->V) return MNB_INVALID_START;
-  int32_t rc;
   if ((rc = check_targets(ctx, mx)) != MNB_OK) return rc;
+  if (rq && rq->n == 0) { ctx->stats = mnb_stats{}; return MNB_SUCCESS; }     // nothing changed: the rows are up to date
   CK(cudaSetDevice(ctx->device));
   const size_t V = ctx->V;
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
@@ -931,12 +966,13 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   }
   int cs = 1; unsigned groups = 1;
   const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
-  rc = mx ? batch_shape(ctx, k_dijkstra_batch<1, true>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups)
+  rc = rq ? batch_shape(ctx, k_dijkstra_batch_repair<1>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups)
+     : mx ? batch_shape(ctx, k_dijkstra_batch<1, true>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups)
           : batch_shape(ctx, k_dijkstra_batch<1>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups);
   if (rc != MNB_OK) return rc;
   if (groups > ctx->dws_groups) {
     ctx->dws = DijkstraBatchBuffers{};        // the smaller workspace goes first: batch_shape has counted its bytes as available
-    ctx->dws_groups = 0;
+    ctx->dws_groups = 0; ctx->dws_marks_clean = false;
     const size_t m = (size_t)groups * V;
     CK(ctx->dws.label.reserve(m)); CK(ctx->dws.mark.reserve(m)); CK(ctx->dws.list0.reserve(m)); CK(ctx->dws.list1.reserve(m));
     CK(ctx->dws.ctl.reserve(groups));
@@ -958,11 +994,24 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
     if ((rc = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return rc;
     a.tg.out = dev ? mx->out : ctx->d_out_dist;
   }
+  DijkstraRepairArgs ra{};
+  if (rq) {
+    static_cast<DijkstraBatchArgs&>(ra) = a;
+    if ((rc = upload_changed(ctx, *rq, groups, ra.chg)) != MNB_OK) return rc;
+    // the repair resets the marks it sets; the batch kernel leaves its marks behind, a new workspace holds anything
+    if (!ctx->dws_marks_clean) CK(cudaMemsetAsync(ctx->dws.mark, 0, sizeof(uint32_t) * (size_t)ctx->dws_groups * V, ctx->stream));
+    if (!dev) {
+      CK(cudaMemcpyAsync(a.out_dist, out_dist, sizeof(float) * (size_t)n * V, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaMemcpyAsync(a.out_pred, out_pred, sizeof(uint32_t) * (size_t)n * V, cudaMemcpyHostToDevice, ctx->stream));
+    }
+  }
+  ctx->dws_marks_clean = false;
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   const unsigned blocks = groups * (unsigned)cs;
   const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
     constexpr int CS = decltype(c)::value;
-    return mx ? launch_cluster(k_dijkstra_batch<CS, true>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
+    return rq ? launch_cluster(k_dijkstra_batch_repair<CS>, ra, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
+         : mx ? launch_cluster(k_dijkstra_batch<CS, true>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
               : launch_cluster(k_dijkstra_batch<CS>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
   });
   if (e != cudaSuccess) { ctx->err = std::string("dijkstra batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
@@ -973,6 +1022,7 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
     if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if ((rc = finish_stats(ctx, groups, 1, ctx->dws.ctl)) != MNB_OK) return rc;
+  ctx->dws_marks_clean = rq != nullptr;      // every wave of the repair has reset its marks (a canceled one too)
   if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
   return MNB_SUCCESS;
 }
@@ -1410,6 +1460,11 @@ int32_t mnb_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_vertex, d
 int32_t mnb_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, float* out_dist,
                            uint32_t* out_pred) {
   return guarded(ctx, [&]() { return impl_dijkstra_batch(ctx, n, seed_vertices, cost_limit, out_dist, out_pred); });
+}
+int32_t mnb_dijkstra_batch_repair(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, double cost_limit, uint32_t n_changed,
+                                  const uint32_t* changed, float* io_dist, uint32_t* io_pred) {
+  const RepairRequest rq{n_changed, changed};
+  return guarded(ctx, [&]() { return impl_dijkstra_batch(ctx, n, seed_vertices, cost_limit, io_dist, io_pred, nullptr, &rq); });
 }
 int32_t mnb_dijkstra_matrix(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_vertices, uint32_t m, const uint32_t* target_vertices,
                             double cost_limit, float* out) {

@@ -778,6 +778,47 @@ struct DijkstraProblemT : TimeAlg {
 };
 using DijkstraProblem = DijkstraProblemT<uint4>;
 
+// ---------------------------------------------------------------------------
+// Dijkstra field repair (k_dijkstra_batch_repair): the same pull on the caller's rows, which hold realizable upper bounds
+// of the new distances from the start.  A band-filtered pull can miss a source beyond the band, so a label never rises:
+// the smaller of the stored and the pulled value stays (in a fresh wave the two are always equal).  The round loop
+// activates on a change of label (REPAIR) and logs every vertex it marks in log[*log_n++] so that the kernel can reset
+// the marks of the wave without a V-sized pass.
+// ---------------------------------------------------------------------------
+struct DijkstraRepairProblem : DijkstraProblemT<float> {
+  static constexpr bool REPAIR = true;
+  uint32_t* log;
+  unsigned int* log_n;
+
+  __device__ __forceinline__ void log_mark(uint32_t x) const { log[atomicAdd(log_n, 1u)] = x; }
+
+  __device__ __forceinline__ bool recompute(uint32_t c, float band_end, float /*goal*/, uint32_t /*round*/, const Label& old, float& nd, float& ntau) {
+    const uint32_t kb = adj_ptr[c], ke = adj_ptr[c + 1];
+    float best = __uint_as_float(INF_BITS), best_du = best; uint32_t best_u = c;
+    for (uint32_t k = kb; k < ke; ++k) {
+      const uint2 nw = __ldg(&adj_nw[k]);
+      const uint32_t u = nw.x;
+      const float du = __ldcg(&state[u]);
+      if (!(du < band_end)) continue;
+      if ((double)__ldg(&cost[u]) > cost_limit) continue;
+      const float tmp = __fadd_rn(du, __uint_as_float(nw.y));
+      if (tmp < best || (tmp == best && __float_as_uint(tmp) != INF_BITS &&
+                         (du < best_du || (du == best_du && u < best_u)))) {
+        best = tmp; best_du = du; best_u = u;
+      }
+    }
+    if (!(best < old.d)) {                 // no better path: the stored label (and, unless tied, its predecessor) stays
+      nd = old.d; ntau = old.d;
+      if (best == old.d && __float_as_uint(best) != INF_BITS && pred[c] != best_u) pred[c] = best_u;
+      return false;
+    }
+    nd = best; ntau = best;
+    store_d(c, nd);
+    pred[c] = best_u;
+    return true;
+  }
+};
+
 
 // ---------------------------------------------------------------------------
 // Dijkstra, 8 lanes per candidate: the adjacency lives in an ELL table, row c = 8 slots x {neighbour, weight bits,
