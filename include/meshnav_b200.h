@@ -288,6 +288,27 @@ int32_t mnb_inflation_update(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, 
                              const mnb_inflation_params* params, float* out_dist, float* out_cost,
                              uint32_t* out_changed /* V */, uint32_t* n_changed);
 
+/* The same result from the part of the map a change can reach.  Arguments and pointer modes are those of
+ * mnb_inflation_update (lethals: the whole new lethal set; duplicates and ids >= V are ignored as there); out_dist and
+ * out_cost are bit-identical to what it returns.  out_changed (room for V ids, may be NULL) lists, ascending, exactly the
+ * vertices whose riskiness entry changed against the previous inflation result on this context -- presence or value
+ * bits, NaN = no entry, NaN equal to NaN -- which is the set to hand to mnb_max_combination_update /
+ * mnb_update_vertex_costs; *n_changed (host) receives the count.
+ * The previous result may come from mnb_inflate, mnb_inflation_update or an earlier repair, with planner calls in
+ * between.  A cluster of that result (a connected component of its finite distances_, linked through shared faces) is
+ * affected when it contains or shares a face with a vertex whose lethal or invalid flag changed; the wave re-runs from
+ * the new lethals of the affected clusters and the new ones outside the old footprint, and again with more clusters while
+ * its footprint touches an unaffected one; every other vertex keeps its bits (DESIGN §4).  Without a previous result, or
+ * with params not bitwise equal to its params, one whole-map wave runs, and so it does when more than half of the old
+ * footprint lies in affected clusters (the call chooses; the changed set is the same tight set).  An unchanged lethal set
+ * and mask run no wave and leave the wave's labels in the workspace as they were.
+ * A repulsive field made valid by mnb_inflation_vector_map stays valid: it is recomputed on the region, and
+ * mnb_inflation_vector_map returns it.  Otherwise mnb_inflation_vector_map needs whole-map labels: it works after a
+ * whole-map wave (and after a call that ran no wave, if it worked before it) and returns MNB_E_STATE after a local one.  Stats: rounds, recomputes and settled summed over the passes; each pass launches three kernels. */
+int32_t mnb_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid /* V or NULL */,
+                             const mnb_inflation_params* params, float* out_dist /* V or NULL */, float* out_cost /* V or NULL */,
+                             uint32_t* out_changed /* V or NULL */, uint32_t* n_changed /* host */);
+
 /* ---- ray casting against the map -------------------------------------------------------------------------------------
  * The shared raycaster of the map (MeshMap::raycaster(), mesh_map.h:318; lvr2::EmbreeRaycaster / BVHRaycaster built at
  * mesh_map.cpp:317-321) as a linear BVH over the faces on the device, built at the first ray call after mnb_set_mesh.

@@ -54,7 +54,7 @@ EXPORTS = [
     "mnb_compute_edge_weights", "mnb_set_costs", "mnb_dijkstra", "mnb_dijkstra_batch", "mnb_cvp", "mnb_cvp_batch", "mnb_cvp_batch_fields",
     "mnb_dijkstra_matrix", "mnb_cvp_matrix", "mnb_dijkstra_batch_repair", "mnb_inflate",
     "mnb_cancel", "mnb_get_stats", "mnb_set_tuning", "mnb_compute_layers", "mnb_get_vertex_normals", "mnb_vector_map", "mnb_cvp_backtrack", "mnb_locate",
-    "mnb_update_vertex_costs", "mnb_get_costs", "mnb_max_combination_update", "mnb_avg_combination_update", "mnb_inflation_update",
+    "mnb_update_vertex_costs", "mnb_get_costs", "mnb_max_combination_update", "mnb_avg_combination_update", "mnb_inflation_update", "mnb_inflation_repair",
     "mnb_inflation_vector_map", "mnb_inflation_vector_at", "mnb_set_repulsive_field",
     "mnb_cast_rays", "mnb_obstacle_update", "mnb_obstacle_reset", "mnb_normal_clearance",
     "mnb_group_create", "mnb_group_destroy", "mnb_group_size", "mnb_group_ctx", "mnb_group_last_error", "mnb_group_set_mesh",
@@ -108,6 +108,8 @@ def load():
     L.mnb_avg_combination_update.argtypes = [vp, u32, vp, vp, vp, vp, u32, vp, vp, vp]
     L.mnb_inflation_update.restype = i32
     L.mnb_inflation_update.argtypes = [vp, vp, u32, vp, C.POINTER(InflationParams), vp, vp, vp, C.POINTER(C.c_uint32)]
+    L.mnb_inflation_repair.restype = i32
+    L.mnb_inflation_repair.argtypes = [vp, vp, u32, vp, C.POINTER(InflationParams), vp, vp, vp, C.POINTER(C.c_uint32)]
     L.mnb_inflation_vector_map.restype = i32; L.mnb_inflation_vector_map.argtypes = [vp, vp]
     L.mnb_inflation_vector_at.restype = i32; L.mnb_inflation_vector_at.argtypes = [vp, u32, vp, vp, vp]
     L.mnb_set_repulsive_field.restype = i32; L.mnb_set_repulsive_field.argtypes = [vp, i32]

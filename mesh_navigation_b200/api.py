@@ -462,6 +462,20 @@ class InflationLayer:
                                           _p(changed), C.byref(n)))
         return dict(dist=dist, cost=cost, changed=changed[:n.value].copy(), **m.stats())
 
+    def repairInflation(self, lethals, invalid=None):
+        """onInputChanged's riskiness from a wave over the lethal clusters the change reaches (mnb_inflation_repair):
+        dist and cost bit-identical to onInputChanged; changed = the vertices whose riskiness entry changed, ascending"""
+        m = self.map
+        le = np.ascontiguousarray(lethals, dtype=np.uint32)
+        inv = None if invalid is None else np.ascontiguousarray(invalid, dtype=np.uint8)
+        dist = np.empty(m.V, dtype=np.float32)
+        cost = np.empty(m.V, dtype=np.float32)
+        changed = np.empty(m.V, dtype=np.uint32)
+        n = C.c_uint32(0)
+        m._check(m.L.mnb_inflation_repair(m._ctx, _p(le), le.size, _p(inv), C.byref(self.config), _p(dist), _p(cost),
+                                          _p(changed), C.byref(n)))
+        return dict(dist=dist, cost=cost, changed=changed[:n.value].copy(), **m.stats())
+
 
 class ObstacleLayer:
     """mesh_layers::ObstacleLayer (obstacle_layer.cpp): the lethal set of the latest point cloud"""

@@ -157,6 +157,62 @@ __device__ __forceinline__ float iv_len(const float* __restrict__ pos, uint32_t 
   return sqrtf(dx * dx + dy * dy + dz * dz);
 }
 
+// The per-vertex bodies of the three kernels, shared with the repair's vertex-list kernels (kernels_infl_repair.cuh).
+// k_infl_vec_lethal keeps its own copy of the first: calling the shared body costs it one register.
+__device__ __forceinline__ void infl_vec_lethal_at(const InflVecArgs a, uint32_t x) {
+  if (x >= a.V) return;
+  float* out = a.vec + 3 * (size_t)x;
+  out[0] = 0.0f; out[1] = 0.0f; out[2] = 0.0f;
+  unsigned long long key[IV_MAXE]; uint8_t ev_face[IV_MAXE];
+  F3 fdir[IV_MAXF];
+  int ne = 0, nf = 0;
+  for (uint32_t k = a.cor_ptr[x]; k < a.cor_ptr[x + 1]; ++k) {
+    const uint32_t f = (uint32_t)a.cor_idx[k].z;
+    const uint32_t fa = a.faces[3 * (size_t)f], fb = a.faces[3 * (size_t)f + 1], fc = a.faces[3 * (size_t)f + 2];
+    const bool la = __uint_as_float(a.ws.state[fa].x) == 0.0f, lb = __uint_as_float(a.ws.state[fb].x) == 0.0f,
+               lc = __uint_as_float(a.ws.state[fc].x) == 0.0f;
+    uint32_t w1, w2, w3;                                       // argument order of waveFrontUpdate (:445-470)
+    if (la && lb && !lc) { w1 = fa; w2 = fb; w3 = fc; }
+    else if (la && !lb && lc) { w1 = fc; w2 = fa; w3 = fb; }
+    else if (!la && lb && lc) { w1 = fb; w2 = fc; w3 = fa; }
+    else continue;
+    const float cand = inflation_candidate(0.0f, 0.0f, iv_len(a.pos, w2, w3), iv_len(a.pos, w1, w3), iv_len(a.pos, w1, w2));
+    if (__float_as_uint(cand) == INF_BITS) continue;           // :271 non-finite update: the call returns before the vectors
+    if (nf >= IV_MAXF) { atomicAdd(&a.flag[1], 1u); return; }
+    const F3 p1 = f3load(a.pos, w1), p2 = f3load(a.pos, w2), p3 = f3load(a.pos, w3);
+    fdir[nf] = f3normalized(F3{(p3.x - p2.x) + (p3.x - p1.x), (p3.y - p2.y) + (p3.y - p1.y), (p3.z - p2.z) + (p3.z - p1.z)});
+    const uint32_t lv[2] = {w1, w2};
+    for (int s = 0; s < 2; ++s) {
+      const uint32_t p = lv[s];                                // the popping lethal vertex
+      if (a.invalid && a.invalid[p]) continue;                 // pops but does not expand (:417)
+      const uint32_t others[2] = {p == w1 ? w2 : w1, w3};
+      for (int t = 0; t < 2; ++t) {
+        const uint32_t q = others[t];
+        uint32_t epos = 0;                                     // position of edge (p,q) among p's edges (ascending edge id)
+        for (uint32_t kk = a.adj_ptr[p]; kk < a.adj_ptr[p + 1]; ++kk) if (a.adj_nbr[kk] == q) { epos = kk - a.adj_ptr[p]; break; }
+        uint32_t side = 0;                                     // an edge lists its faces in ascending id
+        for (uint32_t kk = a.cor_ptr[p]; kk < a.cor_ptr[p + 1]; ++kk) {
+          const int4 ix = a.cor_idx[kk];
+          if ((uint32_t)ix.z != f && ((uint32_t)ix.x == q || (uint32_t)ix.y == q)) { side = (uint32_t)ix.z < f ? 1u : 0u; break; }
+        }
+        key[ne] = ((unsigned long long)p << 32) | ((unsigned long long)epos << 1) | side;
+        ev_face[ne] = (uint8_t)nf; ++ne;
+      }
+    }
+    ++nf;
+  }
+  if (ne == 0) return;
+  F3 v{0.0f, 0.0f, 0.0f};
+  for (int i = 0; i < ne; ++i) {                               // selection sort: <= 96 events, usually 4-16
+    int b = i;
+    for (int j = i + 1; j < ne; ++j) if (key[j] < key[b]) b = j;
+    const unsigned long long kb = key[b]; const uint8_t fbi = ev_face[b];
+    key[b] = key[i]; ev_face[b] = ev_face[i]; key[i] = kb; ev_face[i] = fbi;
+    const F3 d = fdir[fbi];
+    v = f3normalized(F3{v.x + d.x, v.y + d.y, v.z + d.z});
+  }
+  out[0] = v.x; out[1] = v.y; out[2] = v.z;
+}
 __global__ void __launch_bounds__(128) k_infl_vec_lethal(const InflVecArgs a) {
   const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= a.V) return;
@@ -213,8 +269,7 @@ __global__ void __launch_bounds__(128) k_infl_vec_lethal(const InflVecArgs a) {
   out[0] = v.x; out[1] = v.y; out[2] = v.z;
 }
 
-__global__ void __launch_bounds__(128) k_infl_vec_sources(const InflVecArgs a) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void infl_vec_sources_at(const InflVecArgs& a, uint32_t c) {
   if (c >= a.V) return;
   int4 r = make_int4(-1, -1, 0, 0);
   const float d = __uint_as_float(a.ws.state[c].x);
@@ -234,10 +289,11 @@ __global__ void __launch_bounds__(128) k_infl_vec_sources(const InflVecArgs a) {
   }
   a.src[c] = r;
 }
+__global__ void __launch_bounds__(128) k_infl_vec_sources(const InflVecArgs a) {
+  infl_vec_sources_at(a, blockIdx.x * blockDim.x + threadIdx.x);
+}
 
-__global__ void __launch_bounds__(256) k_infl_vec_sweep(const InflVecArgs a) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= a.V) return;
+__device__ __forceinline__ void infl_vec_sweep_at(const InflVecArgs a, uint32_t c) {
   const int4 r = a.src[c];
   if (r.x < 0) return;
   const float d31 = __int_as_float(r.z), d32 = __int_as_float(r.w);
@@ -249,6 +305,11 @@ __global__ void __launch_bounds__(256) k_infl_vec_sweep(const InflVecArgs a) {
     out[0] = v.x; out[1] = v.y; out[2] = v.z;
     a.flag[0] = 1u;
   }
+}
+__global__ void __launch_bounds__(256) k_infl_vec_sweep(const InflVecArgs a) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= a.V) return;
+  infl_vec_sweep_at(a, c);
 }
 
 // InflationLayer::vectorAt(vertices, barycentric_coords) (inflation_layer.cpp:493-521); see oracle inflationVectorAt

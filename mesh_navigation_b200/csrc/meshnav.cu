@@ -26,6 +26,13 @@ using namespace mnb;
 #include "kernels_field.cuh"
 #include "kernels_updates.cuh"
 #include "kernels_raycast.cuh"
+#include "kernels_infl_repair.cuh"
+
+// mnb_inflation_repair runs the whole-map wave when more than this share of the old footprint lies in affected clusters:
+// the local path pays its O(V) passes on top of the wave and, when a new footprint reaches an unaffected cluster, a second
+// pass over everything affected.  On the 5 M bench map (DESIGN §5, H100 at 700 W) the local path took 1.1 ms against
+// 6.6 ms for the full call at a share of 0.0002, 5.4 against 6.7 ms at 0.28 and 10.3 against 6.6 ms at 0.70.
+constexpr double INFL_REPAIR_MAX_SHARE = 0.5;
 
 // default band width of the batched Dijkstra planner in mean edge weights: on the 1 M terrain with 1024 goals 1.5 w was
 // fastest of 1 - 10 w (DESIGN §5)
@@ -116,6 +123,14 @@ struct MeshState : RayCasterState {
   bool infl_labels_valid = false, infl_had_invalid = false, infl_field_valid = false, repulsive_on = false;
   mnb_inflation_params infl_params{}; uint64_t infl_rounds = 0;
   DeviceBuffer<float> d_infl_vec, d_infl_dist; DeviceBuffer<int4> d_infl_src; DeviceBuffer<unsigned int> d_infl_flag;
+  bool infl_field_resident = false;  // the field is the answer of mnb_inflation_vector_map as it stands (a repair kept it)
+  // inflation repair: infl_resident = distances_, riskiness, the lethal set (mnb_ctx::d_lethals, infl_n_lethals) and the
+  // invalid mask of the last inflation are on the device.  The staging of the next set and mask, the cluster ids of the
+  // footprint (built by the first repair after a whole-map wave), four bitmaps of V/32 + 1 words (old lethals, new
+  // lethals, affected clusters, changed riskiness), the seed and region lists and the counters of k_infl_*
+  bool infl_resident = false, infl_cid_valid = false; uint32_t infl_n_lethals = 0;
+  DeviceBuffer<uint32_t> d_infl_lethals_next; DeviceBuffer<uint8_t> d_infl_invalid_next;
+  DeviceBuffer<uint32_t> d_infl_cid, d_infl_bits, d_infl_seeds, d_infl_region; DeviceBuffer<unsigned int> d_infl_cnt;
   // incremental updates
   DeviceBuffer<float> d_prev_risk; bool prev_risk_valid = false;     // riskiness map of the previous inflation (NaN = no entry)
   DeviceBuffer<uint32_t> d_upd_ids; DeviceBuffer<float> d_upd_costs;
@@ -483,13 +498,10 @@ static RepulsiveField repulsive_field_of(mnb_ctx* ctx) {
 
 extern "C" {
 
-static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
-  if (!ctx || !ctx->V) return MNB_E_ARG;
-  if (!ctx->infl_labels_valid) {
-    ctx->err = "mnb_inflation_vector_map needs the labels of the last mnb_inflate / mnb_inflation_update: call it before the next planner call on this context";
-    return MNB_E_STATE;
-  }
-  CK(cudaSetDevice(ctx->device));
+// The repulsive field from the labels of the last inflation wave in the workspace (the wave ran with the invalid mask
+// d_infl_invalid if infl_had_invalid): of every vertex (list null), or of the vertices of a list whose clusters that
+// wave labelled (mnb_inflation_repair) -- the vectors of a cluster depend on sources in that cluster only.
+static int32_t infl_vector_field(mnb_ctx* ctx, const uint32_t* list, uint32_t n, unsigned& launches) {
   const size_t V = ctx->V;
   CK(ctx->d_infl_vec.reserve(3 * V)); CK(ctx->d_infl_src.reserve(V)); CK(ctx->d_infl_flag.reserve(2));
   InflVecArgs a{};
@@ -497,24 +509,51 @@ static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
   a.cor_eid = ctx->d_cor_eid; a.adj_ptr = ctx->d_adj_ptr; a.adj_nbr = ctx->d_adj_nbr; a.invalid = ctx->infl_had_invalid ? ctx->d_infl_invalid.p : nullptr; a.ws = wave_workspace(ctx);
   a.max_distance = (float)ctx->infl_params.inflation_radius; a.vec = ctx->d_infl_vec; a.src = ctx->d_infl_src; a.flag = ctx->d_infl_flag;
   CK(cudaMemsetAsync(ctx->d_infl_flag, 0, 2 * sizeof(unsigned int), ctx->stream));
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  MNB_LAUNCH(k_infl_vec_lethal, (ctx->V + 127) / 128, 128, 0, ctx->stream, a);
-  MNB_LAUNCH(k_infl_vec_sources, (ctx->V + 127) / 128, 128, 0, ctx->stream, a);
+  if (list) {
+    MNB_LAUNCH(k_infl_vec_lethal_list, (n + 127) / 128, 128, 0, ctx->stream, a, list, n);
+    MNB_LAUNCH(k_infl_vec_sources_list, (n + 127) / 128, 128, 0, ctx->stream, a, list, n);
+  } else {
+    MNB_LAUNCH(k_infl_vec_lethal, (ctx->V + 127) / 128, 128, 0, ctx->stream, a);
+    MNB_LAUNCH(k_infl_vec_sources, (ctx->V + 127) / 128, 128, 0, ctx->stream, a);
+  }
   CK(cudaGetLastError());
-  unsigned launches = 2;
+  launches += 2;
   // fixed point over the acyclic source relation: its depth is bounded by the number of rounds the wave took
   const unsigned max_sweeps = (unsigned)ctx->infl_rounds + 8u;
   unsigned int flag[2] = {1u, 0u};
   for (unsigned it = 0; it < max_sweeps && flag[0]; ++it, ++launches) {
     CK(cudaMemsetAsync(ctx->d_infl_flag, 0, sizeof(unsigned int), ctx->stream));
-    MNB_LAUNCH(k_infl_vec_sweep, (ctx->V + 255) / 256, 256, 0, ctx->stream, a);
+    if (list) MNB_LAUNCH(k_infl_vec_sweep_list, (n + 255) / 256, 256, 0, ctx->stream, a, list, n);
+    else MNB_LAUNCH(k_infl_vec_sweep, (ctx->V + 255) / 256, 256, 0, ctx->stream, a);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(flag, ctx->d_infl_flag, sizeof(flag), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
-  CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (flag[1]) { ctx->err = "inflation vector field: a vertex has more than 24 faces with two lethal vertices"; return MNB_E_NOMEM; }
   if (flag[0]) { ctx->err = "inflation vector field did not reach its fixed point"; return MNB_E_STATE; }
+  return MNB_OK;
+}
+
+static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
+  if (!ctx || !ctx->V) return MNB_E_ARG;
+  if (ctx->infl_field_resident) {            // kept up to date by mnb_inflation_repair: no labels needed
+    CK(cudaSetDevice(ctx->device));
+    if (out_vectors) CK(cudaMemcpyAsync(out_vectors, ctx->d_infl_vec, sizeof(float) * 3 * (size_t)ctx->V, out_kind(ctx), ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->stats = mnb_stats{};
+    return MNB_OK;
+  }
+  if (!ctx->infl_labels_valid) {
+    ctx->err = "mnb_inflation_vector_map needs the labels of the last mnb_inflate / mnb_inflation_update: call it before the next planner call on this context";
+    return MNB_E_STATE;
+  }
+  CK(cudaSetDevice(ctx->device));
+  const size_t V = ctx->V;
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  unsigned launches = 0;
+  const int32_t rc = infl_vector_field(ctx, nullptr, 0, launches);
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  if (rc != MNB_OK) return rc;
   if (out_vectors) CK(cudaMemcpyAsync(out_vectors, ctx->d_infl_vec, sizeof(float) * 3 * V, out_kind(ctx), ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, launches, ctx->V);
@@ -1227,6 +1266,46 @@ int32_t mnb_debug_get_label_sides(mnb_ctx* ctx, uint32_t* root, uint32_t* ext, u
 
 }  // extern "C"
 
+// The inputs of an inflation wave: the workspace, the scratch outputs, the lethal list and the invalid mask staged into
+// d_lethals / d_invalid (device copies of the caller's arrays in either pointer mode).
+static int32_t stage_inflation(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid,
+                               DeviceBuffer<uint32_t>& d_lethals, DeviceBuffer<uint8_t>& d_invalid) {
+  int32_t rc;
+  if ((rc = ensure_workspace(ctx, 1)) != MNB_OK) return rc;
+  if ((rc = ensure_out(ctx, (size_t)ctx->V, false)) != MNB_OK) return rc;
+  CK(ctx->d_out_cost.reserve(ctx->V));
+  CK(d_lethals.reserve(n));
+  if (n) CK(cudaMemcpyAsync(d_lethals, lethals, sizeof(uint32_t) * n, in_kind(ctx), ctx->stream));
+  if (invalid) {
+    CK(d_invalid.reserve(ctx->V));
+    CK(cudaMemcpyAsync(d_invalid, invalid, (size_t)ctx->V, in_kind(ctx), ctx->stream));
+  }
+  return MNB_OK;
+}
+
+// one k_inflate launch from a device lethal list (ev0 is recorded just before it when record_start is set)
+static int32_t launch_inflate(mnb_ctx* ctx, const uint32_t* d_lethals, uint32_t n, const uint8_t* d_invalid,
+                              const mnb_inflation_params* params, float* out_dist, float* out_cost, bool record_start) {
+  CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
+  InflateKernelArgs a{};
+  a.V = ctx->V; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx; a.cor_wd = ctx->d_cor_wd; a.cor_eid = ctx->d_cor_eid;
+  a.invalid = d_invalid; a.ws = wave_workspace(ctx); a.lethals = d_lethals; a.n_lethals = n;
+  a.max_distance = (float)params->inflation_radius;      // double -> `const float&` parameter (inflation_layer.cpp:240,450)
+  a.params.inscribed_radius = params->inscribed_radius; a.params.inflation_radius = params->inflation_radius;
+  a.params.lethal_value = params->lethal_value; a.params.inscribed_value = params->inscribed_value;
+  a.params.cost_scaling_factor = params->cost_scaling_factor;
+  a.out_dist = out_dist; a.out_cost = out_cost;
+  a.max_rounds = watchdog_rounds(ctx->V); a.skip_clean = ctx->infl_skip_clean;
+  if (record_start) CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  int infl_per_sm = 1;
+  if (MNB_INFL_MINBLOCKS > 1) {
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&infl_per_sm, k_inflate, ctx->threads, 0));
+    infl_per_sm = std::max(1, std::min(infl_per_sm, (int)MNB_INFL_MINBLOCKS));
+  }
+  CK(launch_cooperative(k_inflate, a, (unsigned)(ctx->sm_count * infl_per_sm), ctx->threads, ctx->stream));
+  return MNB_OK;
+}
+
 // InflationLayer::waveCostInflation; with want_update additionally the update set of InflationLayer::onInputChanged
 static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid,
                             const mnb_inflation_params* params, float* out_dist, float* out_cost, bool want_update,
@@ -1234,39 +1313,17 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
   if (!ctx || !ctx->V || !params || (n && !lethals)) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
   ctx->infl_labels_valid = false;
+  ctx->infl_resident = false; ctx->infl_cid_valid = false; ctx->infl_field_resident = false;
   int32_t rc;
-  if ((rc = ensure_workspace(ctx, 1)) != MNB_OK) return rc;
+  if ((rc = stage_inflation(ctx, lethals, n, invalid, ctx->d_lethals, ctx->d_infl_invalid)) != MNB_OK) return rc;
   const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  if ((rc = ensure_out(ctx, (size_t)ctx->V, false)) != MNB_OK) return rc;
-  CK(ctx->d_out_cost.reserve(ctx->V));
-  CK(ctx->d_lethals.reserve(n));
-  if (n) CK(cudaMemcpyAsync(ctx->d_lethals, lethals, sizeof(uint32_t) * n, in_kind(ctx), ctx->stream));
-  if (invalid) {
-    CK(ctx->d_infl_invalid.reserve(ctx->V));
-    CK(cudaMemcpyAsync(ctx->d_infl_invalid, invalid, (size_t)ctx->V, in_kind(ctx), ctx->stream));
-  }
-  CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
-  InflateKernelArgs a{};
-  a.V = ctx->V; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx; a.cor_wd = ctx->d_cor_wd; a.cor_eid = ctx->d_cor_eid;
-  a.invalid = invalid ? ctx->d_infl_invalid.p : nullptr; a.ws = wave_workspace(ctx); a.lethals = ctx->d_lethals; a.n_lethals = n;
-  a.max_distance = (float)params->inflation_radius;      // double -> `const float&` parameter (inflation_layer.cpp:240,450)
-  a.params.inscribed_radius = params->inscribed_radius; a.params.inflation_radius = params->inflation_radius;
-  a.params.lethal_value = params->lethal_value; a.params.inscribed_value = params->inscribed_value;
-  a.params.cost_scaling_factor = params->cost_scaling_factor;
-  a.out_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist;
-  a.out_cost = (dev && out_cost) ? out_cost : ctx->d_out_cost;
-  a.max_rounds = watchdog_rounds(ctx->V); a.skip_clean = ctx->infl_skip_clean;
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  int infl_per_sm = 1;
-  if (MNB_INFL_MINBLOCKS > 1) {
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&infl_per_sm, k_inflate, ctx->threads, 0));
-    infl_per_sm = std::max(1, std::min(infl_per_sm, (int)MNB_INFL_MINBLOCKS));
-  }
-  CK(launch_cooperative(k_inflate, a, (unsigned)(ctx->sm_count * infl_per_sm), ctx->threads, ctx->stream));
+  float* const o_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist.p;
+  float* const o_cost = (dev && out_cost) ? out_cost : ctx->d_out_cost.p;
+  if ((rc = launch_inflate(ctx, ctx->d_lethals, n, invalid ? ctx->d_infl_invalid.p : nullptr, params, o_dist, o_cost, true)) != MNB_OK) return rc;
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_cost) CK(cudaMemcpyAsync(out_cost, a.out_cost, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_dist) CK(cudaMemcpyAsync(out_dist, o_dist, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_cost) CK(cudaMemcpyAsync(out_cost, o_cost, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
   }
   int32_t rc2 = finish_stats(ctx, 1, 1);
   if (rc2 != MNB_OK) return rc2;
@@ -1277,9 +1334,9 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
     CK(ctx->d_changed.reserve(V)); CK(ctx->d_tile_count.reserve(n_tiles)); CK(ctx->d_total.reserve(1));
     const float* old = ctx->prev_risk_valid ? ctx->d_prev_risk.p : nullptr;
     uint32_t* d_out = (dev && out_changed) ? out_changed : ctx->d_changed;
-    MNB_LAUNCH(k_update_set_count, n_tiles, 256, 0, ctx->stream, (const float*)a.out_cost, old, ctx->V, ctx->d_tile_count);
+    MNB_LAUNCH(k_update_set_count, n_tiles, 256, 0, ctx->stream, (const float*)o_cost, old, ctx->V, ctx->d_tile_count);
     MNB_LAUNCH(k_update_set_scan, 1, 1024, 0, ctx->stream, ctx->d_tile_count, n_tiles, ctx->d_total);
-    MNB_LAUNCH(k_update_set_write, n_tiles, 256, 0, ctx->stream, (const float*)a.out_cost, old, ctx->V, (const unsigned int*)ctx->d_tile_count, d_out);
+    MNB_LAUNCH(k_update_set_write, n_tiles, 256, 0, ctx->stream, (const float*)o_cost, old, ctx->V, (const unsigned int*)ctx->d_tile_count, d_out);
     CK(cudaGetLastError());
     unsigned int total = 0;
     CK(cudaMemcpyAsync(&total, ctx->d_total, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1289,13 +1346,159 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
     ctx->stats.kernel_launches += 3;
   }
   CK(ctx->d_prev_risk.reserve(V));
-  CK(cudaMemcpyAsync(ctx->d_prev_risk, a.out_cost, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->d_prev_risk, o_cost, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->prev_risk_valid = true;
   ctx->infl_labels_valid = true; ctx->infl_had_invalid = invalid != nullptr; ctx->infl_params = *params; ctx->infl_field_valid = false; ctx->infl_rounds = ctx->stats.rounds;
   CK(ctx->d_infl_dist.reserve(V));
-  CK(cudaMemcpyAsync(ctx->d_infl_dist, a.out_dist, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));   // distances_
+  CK(cudaMemcpyAsync(ctx->d_infl_dist, o_dist, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));   // distances_
   CK(cudaStreamSynchronize(ctx->stream));
+  ctx->infl_resident = true; ctx->infl_n_lethals = n;
+  return MNB_OK;
+}
+
+// mnb_inflation_repair (DESIGN §4): a fresh inflation wave from the lethals of the clusters of the resident result that
+// the change can reach, patched into the resident result; everything outside those clusters and the new footprint keeps
+// its bits.  Without a resident result, or with other parameters than it was computed with: one whole-map wave.
+static int32_t impl_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid,
+                                     const mnb_inflation_params* params, float* out_dist, float* out_cost,
+                                     uint32_t* out_changed, uint32_t* n_changed) {
+  if (!ctx || !ctx->V || !params || (n && !lethals) || !n_changed) return MNB_E_ARG;
+  CK(cudaSetDevice(ctx->device));
+  const uint32_t V = ctx->V, W = V / 32 + 1;
+  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  const bool local = ctx->infl_resident && std::memcmp(params, &ctx->infl_params, sizeof(mnb_inflation_params)) == 0;
+  const bool field = ctx->infl_field_valid, has_risk = ctx->prev_risk_valid, labels = ctx->infl_labels_valid;
+  ctx->infl_labels_valid = false;
+  int32_t rc;
+  if ((rc = stage_inflation(ctx, lethals, n, invalid, ctx->d_infl_lethals_next, ctx->d_infl_invalid_next)) != MNB_OK) return rc;
+  CK(ctx->d_infl_bits.reserve(4 * (size_t)W)); CK(ctx->d_infl_cnt.reserve(6));
+  CK(ctx->d_infl_seeds.reserve(std::max(n, 1u))); CK(ctx->d_infl_region.reserve(V));
+  CK(ctx->d_infl_dist.reserve(V)); CK(ctx->d_prev_risk.reserve(V)); CK(ctx->d_infl_cid.reserve(V));
+  const uint32_t n_tiles = (W + BITS_TILE_WORDS - 1) / BITS_TILE_WORDS;
+  CK(ctx->d_changed.reserve(V)); CK(ctx->d_tile_count.reserve(n_tiles)); CK(ctx->d_total.reserve(1));
+  // from here on the resident result is being rewritten: a failure leaves none
+  ctx->infl_resident = false; ctx->prev_risk_valid = false; ctx->infl_field_valid = false; ctx->infl_field_resident = false;
+  uint32_t* const old_bits = ctx->d_infl_bits; uint32_t* const new_bits = old_bits + W;
+  uint32_t* const aff = old_bits + 2 * (size_t)W; uint32_t* const chg = old_bits + 3 * (size_t)W;
+  unsigned int* const d_cnt = ctx->d_infl_cnt;
+  const uint8_t* const new_inv = invalid ? ctx->d_infl_invalid_next.p : nullptr;
+  float* const o_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist.p;
+  float* const o_cost = (dev && out_cost) ? out_cost : ctx->d_out_cost.p;
+  CK(cudaMemsetAsync(old_bits, 0, sizeof(uint32_t) * 4 * (size_t)W, ctx->stream));
+  CK(cudaMemsetAsync(d_cnt, 0, 6 * sizeof(unsigned int), ctx->stream));
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  uint64_t launches = 0, rounds = 0, recomputes = 0, settled = 0, skipped = 0, last_rounds = 0;
+  unsigned int cnt[6] = {0u, 0u, 0u, 0u, 0u, 0u};
+  auto read_cnt = [&]() -> int32_t {
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return MNB_OK;
+  };
+  auto wave = [&](const uint32_t* seeds, uint32_t ns) -> int32_t {   // one pass: k_inflate from `seeds`
+    int32_t r = launch_inflate(ctx, seeds, ns, new_inv, params, o_dist, o_cost, false);
+    if (r != MNB_OK) return r;
+    CK(cudaEventRecord(ctx->ev1, ctx->stream));
+    if ((r = finish_stats(ctx, 1, 1)) != MNB_OK) return r;
+    rounds += ctx->stats.rounds; recomputes += ctx->stats.recomputes; settled += ctx->stats.settled; skipped += ctx->stats.skipped;
+    last_rounds = ctx->stats.rounds; ++launches;
+    return MNB_OK;
+  };
+  bool ran = true;                           // a wave ran: o_dist / o_cost hold its dense output
+  bool whole = !local;                       // the wave is the whole-map one
+  uint32_t n_region = 0;
+  ClusterArgs ca{};
+  ca.V = V; ca.cor_ptr = ctx->d_cor_ptr; ca.cor_idx = ctx->d_cor_idx; ca.dist = ctx->d_infl_dist; ca.cid = ctx->d_infl_cid;
+  if (local) {
+    if (!ctx->infl_cid_valid) {              // the first repair after a whole-map wave: cluster ids of its footprint
+      MNB_LAUNCH(k_cluster_init, (V + 255) / 256, 256, 0, ctx->stream, ca);
+      MNB_LAUNCH(k_cluster_unite, (V + 255) / 256, 256, 0, ctx->stream, ca);
+      MNB_LAUNCH(k_cluster_flatten, (V + 255) / 256, 256, 0, ctx->stream, ca);
+      launches += 3;
+    }
+    ctx->infl_cid_valid = false;
+    InflRepairArgs ra{};
+    ra.V = V; ra.cor_ptr = ctx->d_cor_ptr; ra.cor_idx = ctx->d_cor_idx; ra.cid = ctx->d_infl_cid;
+    ra.old_bits = old_bits; ra.new_bits = new_bits; ra.old_inv = ctx->infl_had_invalid ? ctx->d_infl_invalid.p : nullptr; ra.new_inv = new_inv;
+    ra.aff = aff; ra.lethals = ctx->d_infl_lethals_next; ra.n_lethals = n; ra.seeds = ctx->d_infl_seeds; ra.cnt = d_cnt;
+    if (ctx->infl_n_lethals) { MNB_LAUNCH(k_lethal_bits, (ctx->infl_n_lethals + 255) / 256, 256, 0, ctx->stream, (const uint32_t*)ctx->d_lethals, ctx->infl_n_lethals, V, old_bits); ++launches; }
+    if (n) { MNB_LAUNCH(k_lethal_bits, (n + 255) / 256, 256, 0, ctx->stream, (const uint32_t*)ctx->d_infl_lethals_next, n, V, new_bits); ++launches; }
+    MNB_LAUNCH(k_infl_delta, (V + 255) / 256, 256, 0, ctx->stream, ra);
+    MNB_LAUNCH(k_infl_affected_count, (V + 255) / 256, 256, 0, ctx->stream, ra);
+    launches += 2;
+    if ((rc = read_cnt()) != MNB_OK) return rc;
+    ran = cnt[0] != 0;                       // nothing changed: no wave
+    whole = ran && (double)cnt[5] > INFL_REPAIR_MAX_SHARE * (double)cnt[4];
+    // passes: the seeds of the affected clusters, their wave, the merge check; a new footprint that touches an unaffected
+    // cluster makes it affected, so the set of affected clusters only grows and the loop ends
+    for (bool again = ran && !whole; again;) {
+      CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned int), ctx->stream));
+      if (n) { MNB_LAUNCH(k_infl_seeds, (n + 255) / 256, 256, 0, ctx->stream, ra); ++launches; }
+      if ((rc = read_cnt()) != MNB_OK) return rc;
+      if ((rc = wave(ctx->d_infl_seeds, cnt[1])) != MNB_OK) return rc;
+      MNB_LAUNCH(k_infl_merge_check, (V + 255) / 256, 256, 0, ctx->stream, ra, (const float*)o_dist);
+      ++launches;
+      if ((rc = read_cnt()) != MNB_OK) return rc;
+      again = cnt[2] != 0;
+    }
+  }
+  if (whole && (rc = wave(ctx->d_infl_lethals_next, n)) != MNB_OK) return rc;
+  if (ran) {
+    InflPatchArgs pa{};
+    pa.V = V; pa.all = whole ? 1 : 0; pa.aff = aff; pa.cid = whole ? nullptr : ctx->d_infl_cid.p;
+    pa.out_dist = o_dist; pa.out_cost = o_cost; pa.res_dist = ctx->d_infl_dist; pa.res_risk = ctx->d_prev_risk;
+    pa.has_risk = local || has_risk; pa.chg_bits = chg; pa.region = ctx->d_infl_region; pa.n_region = d_cnt + 3;
+    MNB_LAUNCH(k_infl_patch, (V + 255) / 256, 256, 0, ctx->stream, pa);
+    ++launches;
+    if ((rc = read_cnt()) != MNB_OK) return rc;
+    n_region = cnt[3];
+    if (!whole && n_region) {                // cluster ids of the region: the components of the new footprint
+      ca.list = ctx->d_infl_region; ca.n = n_region;
+      MNB_LAUNCH(k_cluster_unite, (n_region + 255) / 256, 256, 0, ctx->stream, ca);
+      MNB_LAUNCH(k_cluster_flatten, (n_region + 255) / 256, 256, 0, ctx->stream, ca);
+      launches += 2;
+    }
+    ctx->infl_cid_valid = !whole;
+  } else {
+    ctx->infl_cid_valid = true;
+  }
+  // the changed set: ordered compaction of the bits the patch set
+  uint32_t* const d_out = (dev && out_changed) ? out_changed : ctx->d_changed.p;
+  MNB_LAUNCH(k_bits_count, n_tiles, 256, 0, ctx->stream, (const uint32_t*)chg, W, ctx->d_tile_count);
+  MNB_LAUNCH(k_update_set_scan, 1, 1024, 0, ctx->stream, ctx->d_tile_count, n_tiles, ctx->d_total);
+  MNB_LAUNCH(k_bits_write, n_tiles, 256, 0, ctx->stream, (const uint32_t*)chg, W, (const unsigned int*)ctx->d_tile_count, d_out);
+  launches += 3;
+  CK(cudaGetLastError());
+  // the new set and mask are the resident ones from here on
+  std::swap(ctx->d_lethals, ctx->d_infl_lethals_next);
+  if (invalid) std::swap(ctx->d_infl_invalid, ctx->d_infl_invalid_next);
+  ctx->infl_n_lethals = n; ctx->infl_had_invalid = invalid != nullptr; ctx->infl_params = *params;
+  if (ran) ctx->infl_rounds = last_rounds;
+  // a whole-map wave leaves whole-map labels in the workspace; without a wave the labels there are still current
+  ctx->infl_labels_valid = whole || (!ran && labels);
+  if (field && ran && (whole || n_region)) {   // the repulsive field of the region (of every vertex after a whole-map wave)
+    unsigned fl = 0;
+    if ((rc = infl_vector_field(ctx, whole ? nullptr : ctx->d_infl_region.p, n_region, fl)) != MNB_OK) return rc;
+    launches += fl;
+  }
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  unsigned int total = 0;
+  CK(cudaMemcpyAsync(&total, ctx->d_total, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  *n_changed = total;
+  if (!dev && out_changed && total) CK(cudaMemcpyAsync(out_changed, d_out, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+  const float* src_dist = ran ? o_dist : ctx->d_infl_dist.p;
+  const float* src_cost = ran ? o_cost : ctx->d_prev_risk.p;
+  if (out_dist && out_dist != src_dist) CK(cudaMemcpyAsync(out_dist, src_dist, sizeof(float) * (size_t)V, out_kind(ctx), ctx->stream));
+  if (out_cost && out_cost != src_cost) CK(cudaMemcpyAsync(out_cost, src_cost, sizeof(float) * (size_t)V, out_kind(ctx), ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+  ctx->stats = mnb_stats{};
+  ctx->stats.rounds = rounds; ctx->stats.recomputes = recomputes; ctx->stats.settled = settled; ctx->stats.skipped = skipped;
+  ctx->stats.kernel_launches = launches; ctx->stats.kernel_ms = ms;
+  ctx->infl_resident = true; ctx->prev_risk_valid = true;
+  ctx->infl_field_valid = field; ctx->infl_field_resident = field;
   return MNB_OK;
 }
 
@@ -1502,6 +1705,11 @@ int32_t mnb_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32_t* out_
 }
 int32_t mnb_vector_map(mnb_ctx* ctx, const uint32_t* pred, const float* direction, const int32_t* cutting_face, float* out_vec) {
   return guarded(ctx, [&]() { return impl_vector_map(ctx, pred, direction, cutting_face, out_vec); });
+}
+int32_t mnb_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, const uint8_t* invalid,
+                             const mnb_inflation_params* params, float* out_dist, float* out_cost, uint32_t* out_changed,
+                             uint32_t* n_changed) {
+  return guarded(ctx, [&]() { return impl_inflation_repair(ctx, lethals, n, invalid, params, out_dist, out_cost, out_changed, n_changed); });
 }
 int32_t mnb_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
   return guarded(ctx, [&]() { return impl_inflation_vector_map(ctx, out_vectors); });
