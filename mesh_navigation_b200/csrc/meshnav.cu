@@ -184,6 +184,70 @@ struct mnb_ctx : MeshState {
     }                                                                              \
   } while (0)
 
+// The caller's arrays of one call in the pointer mode (mnb_set_pointer_mode).  In device-pointer mode the kernels get the
+// caller's arrays.  In host-pointer mode they get device staging: in() copies an input there when it is declared, out()
+// queues the copy of an output back, and copy_back() issues the copies queued so far after the launch, in the order the
+// outputs were declared, on ctx->stream.  A DeviceBuffer staging is reserved only when it is used; a raw one is the
+// caller's to reserve.  NULL arrays stay NULL, except that needed() falls back to the staging in both modes for an
+// output the call reads itself.  The first error stops all further work; status() reports it.
+class CallerArrays {
+ public:
+  explicit CallerArrays(mnb_ctx* ctx) : stream_(ctx->stream), dev_(ctx->ptr_mode == MNB_PTR_DEVICE) {}
+  bool device() const { return dev_; }
+  cudaError_t status() const { return err_; }
+
+  template <class T> const T* in(const T* caller, T* staging, size_t n) {
+    if (!caller || dev_) return caller;
+    return ok() && run(cudaMemcpyAsync(staging, caller, sizeof(T) * n, cudaMemcpyHostToDevice, stream_)) ? staging : nullptr;
+  }
+  template <class T> const T* in(const T* caller, DeviceBuffer<T>& staging, size_t n) {
+    if (!caller || dev_) return caller;
+    return ok() && run(staging.reserve(n)) ? in(caller, staging.p, n) : nullptr;
+  }
+  // an output of n elements; with `late` it has n * *late elements, read when copy_back() runs (a list whose length
+  // the call reads back)
+  template <class T> T* out(T* caller, T* staging, size_t n, const uint32_t* late = nullptr) {
+    if (!caller || dev_) return caller;
+    if (!ok()) return nullptr;
+    queued_.push_back(Copy{caller, staging, sizeof(T), n, late});
+    return staging;
+  }
+  template <class T> T* out(T* caller, DeviceBuffer<T>& staging, size_t n) {
+    if (!caller || dev_) return caller;
+    return ok() && run(staging.reserve(n)) ? out(caller, staging.p, n) : nullptr;
+  }
+  template <class T> T* needed(T* caller, T* staging, size_t n, const uint32_t* late = nullptr) {
+    return caller ? out(caller, staging, n, late) : staging;
+  }
+  template <class T> T* inout(T* caller, DeviceBuffer<T>& staging, size_t n) {
+    return in((const T*)caller, staging, n) ? out(caller, staging.p, n) : nullptr;
+  }
+  cudaError_t copy_back() {
+    for (const Copy& c : queued_) {
+      const size_t n = c.late ? (size_t)*c.late * c.n : c.n;
+      if (n && !run(cudaMemcpyAsync(c.dst, c.src, c.elem * n, cudaMemcpyDeviceToHost, stream_))) break;
+    }
+    queued_.clear();
+    return err_;
+  }
+  // copies between the caller's arrays and context arrays in either mode
+  template <class T> cudaError_t copy_in(T* dst, const T* caller, size_t n) {
+    return cudaMemcpyAsync(dst, caller, sizeof(T) * n, dev_ ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream_);
+  }
+  template <class T> cudaError_t copy_out(T* caller, const T* src, size_t n) {
+    return cudaMemcpyAsync(caller, src, sizeof(T) * n, dev_ ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_);
+  }
+
+ private:
+  struct Copy { void* dst; const void* src; size_t elem, n; const uint32_t* late; };
+  bool ok() const { return err_ == cudaSuccess; }
+  bool run(cudaError_t e) { err_ = e; return ok(); }
+  cudaStream_t stream_;
+  bool dev_;
+  cudaError_t err_ = cudaSuccess;
+  std::vector<Copy> queued_;
+};
+
 static void free_raycaster(mnb_ctx* c) { static_cast<RayCasterState&>(*c) = RayCasterState{}; }
 static void free_mesh(mnb_ctx* c) { static_cast<MeshState&>(*c) = MeshState{}; }
 
@@ -212,6 +276,18 @@ static int32_t ensure_workspace(mnb_ctx* ctx, uint32_t groups) {
   CK(w.pool.reserve((size_t)groups * ws_pool_cap(ctx->V)));
   CK(w.ctl.reserve(groups));
   ctx->ws_groups = groups;
+  return MNB_OK;
+}
+
+static int32_t ensure_dijkstra_workspace(mnb_ctx* ctx, uint32_t groups) {
+  if (groups <= ctx->dws_groups) return MNB_OK;
+  DijkstraBatchBuffers& w = ctx->dws;
+  w = DijkstraBatchBuffers{};        // the smaller workspace goes first: batch_shape has counted its bytes as available
+  ctx->dws_groups = 0; ctx->dws_marks_clean = false;
+  const size_t n = (size_t)groups * ctx->V;
+  CK(w.label.reserve(n)); CK(w.mark.reserve(n)); CK(w.list0.reserve(n)); CK(w.list1.reserve(n));
+  CK(w.ctl.reserve(groups));
+  ctx->dws_groups = groups;
   return MNB_OK;
 }
 
@@ -399,13 +475,10 @@ int32_t mnb_get_edges(mnb_ctx* ctx, uint32_t* out_edges) {
   return MNB_OK;
 }
 
-static cudaMemcpyKind in_kind(mnb_ctx* c) { return c->ptr_mode == MNB_PTR_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice; }
-static cudaMemcpyKind out_kind(mnb_ctx* c) { return c->ptr_mode == MNB_PTR_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice; }
-
 int32_t mnb_get_edge_distances(mnb_ctx* ctx, float* out) {
   if (!ctx || !out || !ctx->V) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
-  CK(cudaMemcpyAsync(out, ctx->d_edge_dist, sizeof(float) * (size_t)ctx->E, out_kind(ctx), ctx->stream));
+  CK(CallerArrays(ctx).copy_out(out, ctx->d_edge_dist.p, ctx->E));
   CK(cudaStreamSynchronize(ctx->stream));
   return MNB_OK;
 }
@@ -455,12 +528,13 @@ static int32_t ensure_adj_tables(mnb_ctx* ctx) {
 static int32_t impl_compute_edge_weights(mnb_ctx* ctx, const float* vertex_costs, double edge_cost_factor, float* out_w) {
   if (!ctx || !vertex_costs || !ctx->V) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
-  CK(cudaMemcpyAsync(ctx->d_cost, vertex_costs, sizeof(float) * (size_t)ctx->V, in_kind(ctx), ctx->stream));
+  CallerArrays io(ctx);
+  CK(io.copy_in(ctx->d_cost.p, vertex_costs, ctx->V));
   MNB_LAUNCH(k_edge_weights, (ctx->E + 255) / 256, 256, 0, ctx->stream, ctx->d_cost, ctx->d_edges, ctx->d_edge_dist, edge_cost_factor, ctx->E, ctx->d_edge_w);
   CK(cudaGetLastError());
   int32_t rc = install_weights(ctx);
   if (rc != MNB_OK) return rc;
-  if (out_w) CK(cudaMemcpyAsync(out_w, ctx->d_edge_w, sizeof(float) * (size_t)ctx->E, out_kind(ctx), ctx->stream));
+  if (out_w) CK(io.copy_out(out_w, ctx->d_edge_w.p, ctx->E));
   CK(cudaStreamSynchronize(ctx->stream));
   return MNB_OK;
 }
@@ -468,9 +542,10 @@ static int32_t impl_compute_edge_weights(mnb_ctx* ctx, const float* vertex_costs
 static int32_t impl_set_costs(mnb_ctx* ctx, const float* vertex_costs, const float* edge_weights, const uint8_t* invalid) {
   if (!ctx || !vertex_costs || !edge_weights || !ctx->V) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
-  CK(cudaMemcpyAsync(ctx->d_cost, vertex_costs, sizeof(float) * (size_t)ctx->V, in_kind(ctx), ctx->stream));
-  CK(cudaMemcpyAsync(ctx->d_edge_w, edge_weights, sizeof(float) * (size_t)ctx->E, in_kind(ctx), ctx->stream));
-  if (invalid) CK(cudaMemcpyAsync(ctx->d_invalid, invalid, (size_t)ctx->V, in_kind(ctx), ctx->stream));
+  CallerArrays io(ctx);
+  CK(io.copy_in(ctx->d_cost.p, vertex_costs, ctx->V));
+  CK(io.copy_in(ctx->d_edge_w.p, edge_weights, ctx->E));
+  if (invalid) CK(io.copy_in(ctx->d_invalid.p, invalid, ctx->V));
   ctx->has_invalid = invalid != nullptr;
   int32_t rc = install_weights(ctx);
   if (rc != MNB_OK) return rc;
@@ -538,7 +613,7 @@ static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
   if (!ctx || !ctx->V) return MNB_E_ARG;
   if (ctx->infl_field_resident) {            // kept up to date by mnb_inflation_repair: no labels needed
     CK(cudaSetDevice(ctx->device));
-    if (out_vectors) CK(cudaMemcpyAsync(out_vectors, ctx->d_infl_vec, sizeof(float) * 3 * (size_t)ctx->V, out_kind(ctx), ctx->stream));
+    if (out_vectors) CK(CallerArrays(ctx).copy_out(out_vectors, ctx->d_infl_vec.p, 3 * (size_t)ctx->V));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->stats = mnb_stats{};
     return MNB_OK;
@@ -554,7 +629,7 @@ static int32_t impl_inflation_vector_map(mnb_ctx* ctx, float* out_vectors) {
   const int32_t rc = infl_vector_field(ctx, nullptr, 0, launches);
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   if (rc != MNB_OK) return rc;
-  if (out_vectors) CK(cudaMemcpyAsync(out_vectors, ctx->d_infl_vec, sizeof(float) * 3 * V, out_kind(ctx), ctx->stream));
+  if (out_vectors) CK(CallerArrays(ctx).copy_out(out_vectors, ctx->d_infl_vec.p, 3 * V));
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, launches, ctx->V);
   ctx->stats.rounds = ctx->infl_rounds;
@@ -574,17 +649,15 @@ static int32_t impl_inflation_vector_at(mnb_ctx* ctx, uint32_t n, const uint32_t
   if (!ctx->infl_field_valid) { ctx->err = "mnb_inflation_vector_at needs mnb_inflation_vector_map first"; return MNB_E_STATE; }
   for (uint32_t i = 0; ctx->ptr_mode == MNB_PTR_HOST && i < n; ++i) if (faces_q[i] >= ctx->F) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  CallerArrays io(ctx);
   DeviceBuffer<uint32_t> d_f; DeviceBuffer<float> d_b, d_o;      // host-pointer mode: device copies for this call
-  if (!dev) {
-    CK(d_f.reserve((size_t)n)); CK(d_b.reserve(3 * (size_t)n)); CK(d_o.reserve(3 * (size_t)n));
-    CK(cudaMemcpyAsync(d_f, faces_q, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(d_b, bary, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  MNB_LAUNCH(k_inflation_vector_at, (n + 127) / 128, 128, 0, ctx->stream, repulsive_field_of(ctx), (const uint32_t*)ctx->d_faces, n,
-             dev ? faces_q : (const uint32_t*)d_f, dev ? bary : (const float*)d_b, dev ? out : d_o);
+  const uint32_t* const f = io.in(faces_q, d_f, n);
+  const float* const b = io.in(bary, d_b, 3 * (size_t)n);
+  float* const o = io.out(out, d_o, 3 * (size_t)n);
+  CK(io.status());
+  MNB_LAUNCH(k_inflation_vector_at, (n + 127) / 128, 128, 0, ctx->stream, repulsive_field_of(ctx), (const uint32_t*)ctx->d_faces, n, f, b, o);
   CK(cudaGetLastError());
-  if (!dev) CK(cudaMemcpyAsync(out, d_o, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(io.copy_back());
   CK(cudaStreamSynchronize(ctx->stream));
   return MNB_OK;
 }
@@ -673,6 +746,26 @@ static int32_t batch_shape(mnb_ctx* ctx, void (*kern)(const KArgs), uint32_t n, 
   return MNB_OK;
 }
 
+// One batch of n waves (mnb_cvp_batch_fields, mnb_dijkstra_batch): kernel(std::integral_constant<int, CS>()) is the
+// kernel at cluster size CS.  Its one-CTA form sizes the launch (batch_shape), prepare(groups) grows the workspace and
+// fills args, and the launch at the chosen cluster size is timed by ev0 / ev1.
+template <class Kernel, class KArgs, class Prepare>
+static int32_t run_batch(mnb_ctx* ctx, Kernel kernel, const KArgs& args, uint32_t n, size_t per_group, uint32_t current,
+                         const char* what, Prepare prepare, unsigned* groups_out) {
+  int cs = 1; unsigned groups = 1;
+  int32_t rc = batch_shape(ctx, kernel(std::integral_constant<int, 1>()), n, per_group, current, what, &cs, &groups);
+  if (rc != MNB_OK || (rc = prepare(groups)) != MNB_OK) return rc;
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  const unsigned blocks = groups * (unsigned)cs;
+  const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
+    return launch_cluster(kernel(c), args, decltype(c)::value, blocks, MNB_BATCH_THREADS, ctx->stream);
+  });
+  if (e != cudaSuccess) { ctx->err = std::string(what) + " batch launch: " + cudaGetErrorString(e); return MNB_E_CUDA; }
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  *groups_out = groups;
+  return MNB_OK;
+}
+
 static int32_t finish_stats(mnb_ctx* ctx, unsigned groups, unsigned launches, const GroupCtl* ctl = nullptr) {
   std::vector<GroupCtl> h(groups);
   CK(cudaMemcpyAsync(h.data(), ctl ? ctl : ctx->ws.ctl, sizeof(GroupCtl) * groups, cudaMemcpyDeviceToHost, ctx->stream));
@@ -754,13 +847,6 @@ static int32_t upload_changed(mnb_ctx* ctx, const RepairRequest& rq, unsigned gr
   return MNB_OK;
 }
 
-// host-pointer mode: the [n][m] matrix from its device staging (d_out_dist) into the caller's array
-static int32_t copy_matrix_out(mnb_ctx* ctx, uint32_t n, const MatrixRequest* mx) {
-  if (mx && ctx->ptr_mode != MNB_PTR_DEVICE)
-    CK(cudaMemcpyAsync(mx->out, ctx->d_out_dist, sizeof(float) * n * (size_t)mx->m, cudaMemcpyDeviceToHost, ctx->stream));
-  return MNB_OK;
-}
-
 static void fill_cvp_args(mnb_ctx* ctx, CvpKernelArgs& a) {
   a.V = ctx->V; a.pos = ctx->d_pos; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx;
   a.cor_w = ctx->d_cor_w; a.ell_idx = ctx->d_ell_idx; a.ell_w = ctx->d_ell_w; a.ell_geo = ctx->d_ell_geo; a.cost = ctx->d_cost; a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = wave_workspace(ctx);
@@ -781,8 +867,13 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   int32_t rc;
   if ((rc = ensure_workspace(ctx, 1)) != MNB_OK) return rc;
   if ((rc = ensure_seeds(ctx, 1)) != MNB_OK) return rc;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  if ((rc = ensure_out(ctx, dev ? 0 : (size_t)ctx->V, true)) != MNB_OK) return rc;
+  // every row is produced without the caller's array too: the outcome code and mnb_cvp_backtrack read them
+  CallerArrays io(ctx);
+  if ((rc = ensure_out(ctx, (io.device() && out_dist) ? 0 : (size_t)ctx->V, true)) != MNB_OK) return rc;
+  float* const o_dist = io.needed(out_dist, ctx->d_out_dist.p, ctx->V);
+  uint32_t* const o_pred = io.needed(out_pred, ctx->d_out_pred.p, ctx->V);
+  float* const o_dir = io.needed(out_direction, ctx->d_out_dir.p, ctx->V);
+  int32_t* const o_cut = io.needed(out_cut, ctx->d_out_cut.p, ctx->V);
   if (ctx->h_cancel) *ctx->h_cancel = 0;     // cvp:679 "reset cancel planning"
   ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
   CK(cudaMemcpyAsync(ctx->d_seed_faces, &seed_face, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -793,12 +884,7 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   fill_cvp_args(ctx, a);
   a.n_queries = 1; a.robot_face = robot_face; a.cost_limit = cost_limit; a.goal_dist_offset = goal_dist_offset;
   a.sweeps = ctx->sweeps;
-  a.out_dist = dev ? out_dist : ctx->d_out_dist;
-  // aux outputs are always produced for a single plan (the outcome code needs predecessors_)
-  a.out_pred = (dev && out_pred) ? out_pred : ctx->d_out_pred;
-  a.out_dir = (dev && out_direction) ? out_direction : ctx->d_out_dir;
-  a.out_cut = (dev && out_cut) ? out_cut : ctx->d_out_cut;
-  if (dev && !out_dist) { if ((rc = ensure_out(ctx, (size_t)ctx->V, true)) != MNB_OK) return rc; a.out_dist = ctx->d_out_dist; }
+  a.out_dist = o_dist; a.out_pred = o_pred; a.out_dir = o_dir; a.out_cut = o_cut;
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   if (ctx->cluster == -1) {
     a.delta = ctx->grid_delta;
@@ -819,12 +905,7 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   MNB_LAUNCH(k_cvp_epilogue, (ctx->V + 255) / 256, 256, 0, ctx->stream, a, ctx->ws.ctl);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_direction) CK(cudaMemcpyAsync(out_direction, a.out_dir, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_cut) CK(cudaMemcpyAsync(out_cut, a.out_cut, sizeof(int32_t) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   // outcome (cvp:888-918)
   uint32_t rf[3] = {0, 0, 0}, rp[3] = {0, 0, 0};
   if (robot_face >= 0) {
@@ -861,59 +942,45 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
   int32_t rc;
   if ((rc = check_targets(ctx, mx)) != MNB_OK) return rc;
   CK(cudaSetDevice(ctx->device));
-  const size_t V = ctx->V, rows = (size_t)n * V;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  const size_t rows = (size_t)n * ctx->V;
   const bool fields = out_pred || out_dir || out_cut;
   if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
-  if (mx && !dev && (rc = ensure_out(ctx, (size_t)n * mx->m, false)) != MNB_OK) return rc;
-  if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized; the
-                       // single plan's outputs stay untouched for mnb_cvp_backtrack / mnb_vector_map)
-    if (out_dist && (rc = ensure_out(ctx, rows, false)) != MNB_OK) return rc;
-    if (out_pred) CK(ctx->d_batch_pred.reserve(rows));
-    if (out_dir) CK(ctx->d_batch_dir.reserve(rows));
-    if (out_cut) CK(ctx->d_batch_cut.reserve(rows));
-  }
-  int cs = 1; unsigned groups = 1;
-  rc = mx ? batch_shape(ctx, k_cvp_batch<1, false, CvpMatrixArgs>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
-     : fields ? batch_shape(ctx, k_cvp_batch<1, true>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups)
-              : batch_shape(ctx, k_cvp_batch<1, false>, n, ws_bytes_per_group(ctx->V), ctx->ws_groups, "CVP", &cs, &groups);
-  if (rc != MNB_OK) return rc;
-  if ((rc = ensure_workspace(ctx, groups)) != MNB_OK) return rc;
-  if (ctx->h_cancel) *ctx->h_cancel = 0;
-  ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
-  CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_faces, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
-  CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+  // host-pointer staging, reserved before the workspace is sized; the single plan's outputs stay untouched for
+  // mnb_cvp_backtrack / mnb_vector_map
+  CallerArrays io(ctx);
+  float* const o_matrix = mx ? io.out(mx->out, ctx->d_out_dist, (size_t)n * mx->m) : nullptr;
+  float* const o_dist = io.out(out_dist, ctx->d_out_dist, rows);
+  uint32_t* const o_pred = io.out(out_pred, ctx->d_batch_pred, rows);
+  float* const o_dir = io.out(out_dir, ctx->d_batch_dir, rows);
+  int32_t* const o_cut = io.out(out_cut, ctx->d_batch_cut, rows);
+  CK(io.status());
   CvpMatrixArgs a{};
-  fill_cvp_args(ctx, a);
-  a.n_queries = n; a.robot_face = -1; a.cost_limit = cost_limit; a.goal_dist_offset = 0.0;
-  a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
-  a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
-  a.out_dir = !out_dir ? nullptr : (dev ? out_dir : ctx->d_batch_dir);
-  a.out_cut = !out_cut ? nullptr : (dev ? out_cut : ctx->d_batch_cut);
-  if (mx) {
-    if ((rc = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return rc;
-    a.tg.out = dev ? mx->out : ctx->d_out_dist;
-  }
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  const unsigned blocks = groups * (unsigned)cs;
-  const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
-    constexpr int CS = decltype(c)::value;
-    const CvpKernelArgs& b = a;
-    return mx ? launch_cluster(k_cvp_batch<CS, false, CvpMatrixArgs>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
-         : fields ? launch_cluster(k_cvp_batch<CS, true>, b, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
-                  : launch_cluster(k_cvp_batch<CS, false>, b, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
-  });
-  if (e != cudaSuccess) { ctx->err = std::string("cvp batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
-  CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if ((rc = copy_matrix_out(ctx, n, mx)) != MNB_OK) return rc;
-  if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * rows, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * rows, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_dir) CK(cudaMemcpyAsync(out_dir, a.out_dir, sizeof(float) * rows, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_cut) CK(cudaMemcpyAsync(out_cut, a.out_cut, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  auto prepare = [&](unsigned groups) -> int32_t {
+    int32_t r;
+    if ((r = ensure_workspace(ctx, groups)) != MNB_OK) return r;
+    if (ctx->h_cancel) *ctx->h_cancel = 0;
+    ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
+    CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_faces, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
+    CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+    fill_cvp_args(ctx, a);
+    a.n_queries = n; a.robot_face = -1; a.cost_limit = cost_limit; a.goal_dist_offset = 0.0;
+    a.out_dist = o_dist; a.out_pred = o_pred; a.out_dir = o_dir; a.out_cut = o_cut;
+    if (mx) {
+      if ((r = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return r;
+      a.tg.out = o_matrix;
+    }
+    return MNB_OK;
+  };
+  const size_t per_group = ws_bytes_per_group(ctx->V);
+  const CvpKernelArgs& b = a;
+  unsigned groups = 1;
+  rc = mx ? run_batch(ctx, [](auto c) { return k_cvp_batch<decltype(c)::value, false, CvpMatrixArgs>; }, a, n, per_group, ctx->ws_groups, "CVP", prepare, &groups)
+     : fields ? run_batch(ctx, [](auto c) { return k_cvp_batch<decltype(c)::value, true>; }, b, n, per_group, ctx->ws_groups, "CVP", prepare, &groups)
+              : run_batch(ctx, [](auto c) { return k_cvp_batch<decltype(c)::value, false>; }, b, n, per_group, ctx->ws_groups, "CVP", prepare, &groups);
+  if (rc != MNB_OK) return rc;
+  CK(io.copy_back());
   if ((rc = finish_stats(ctx, groups, 1)) != MNB_OK) return rc;
   if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
   return MNB_SUCCESS;
@@ -928,7 +995,6 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   CK(cudaSetDevice(ctx->device));
   int32_t rc;
   if ((rc = ensure_workspace(ctx, 1)) != MNB_OK) return rc;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   if ((rc = ensure_out(ctx, (size_t)ctx->V, true)) != MNB_OK) return rc;
   if (ctx->h_cancel) *ctx->h_cancel = 0;     // dijkstra:238
   ctx->infl_labels_valid = false;
@@ -938,17 +1004,15 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   a.V = ctx->V; a.adj_ptr = ctx->d_adj_ptr; a.adj_nw = ctx->d_adj_nw; a.cost = ctx->d_cost;
   a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = wave_workspace(ctx); a.seed_vertex = seed_vertex;
   a.robot_vertex = robot_vertex; a.cost_limit = cost_limit; a.goal_dist_offset = goal_dist_offset; a.delta = ctx->delta;
-  a.out_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist;
-  a.out_pred = (dev && out_pred) ? out_pred : ctx->d_out_pred;
+  CallerArrays io(ctx);         // both rows are produced without the caller's arrays too: the outcome code reads them
+  a.out_dist = io.needed(out_dist, ctx->d_out_dist.p, ctx->V);
+  a.out_pred = io.needed(out_pred, ctx->d_out_pred.p, ctx->V);
   a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V);
   if (robot_vertex >= 0 && (uint32_t)robot_vertex == seed_vertex) {   // dijkstra:252-255: "start == goal" returns before the wave
     // the reference has cleared its maps by then (:241-249): distances +inf (seed 0), every vertex its own predecessor
     MNB_LAUNCH(k_dijkstra_trivial, (ctx->V + 255) / 256, 256, 0, ctx->stream, ctx->V, seed_vertex, a.out_dist, a.out_pred);
     CK(cudaGetLastError());
-    if (!dev) {
-      if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-      if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    }
+    CK(io.copy_back());
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->stats = mnb_stats{}; ctx->stats.kernel_launches = 1;
     return MNB_SUCCESS;
@@ -967,10 +1031,7 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   }
   if (e != cudaSuccess) { ctx->err = std::string("dijkstra launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   uint32_t rp = 0;
   if (robot_vertex >= 0) CK(cudaMemcpyAsync(&rp, a.out_pred + robot_vertex, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   if ((rc = finish_stats(ctx, 1, 1)) != MNB_OK) return rc;
@@ -995,71 +1056,48 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
   if ((rc = check_targets(ctx, mx)) != MNB_OK) return rc;
   if (rq && rq->n == 0) { ctx->stats = mnb_stats{}; return MNB_SUCCESS; }     // nothing changed: the rows are up to date
   CK(cudaSetDevice(ctx->device));
-  const size_t V = ctx->V;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  const size_t V = ctx->V, rows = (size_t)n * V;
   if ((rc = ensure_seeds(ctx, n)) != MNB_OK) return rc;
-  if (mx && !dev && (rc = ensure_out(ctx, (size_t)n * mx->m, false)) != MNB_OK) return rc;
-  if (!dev) {          // host-pointer mode: device rows to copy back from (allocated before the workspace is sized)
-    if (out_dist && (rc = ensure_out(ctx, (size_t)n * V, false)) != MNB_OK) return rc;
-    if (out_pred) CK(ctx->d_batch_pred.reserve((size_t)n * V));
-  }
-  int cs = 1; unsigned groups = 1;
-  const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
-  rc = rq ? batch_shape(ctx, k_dijkstra_batch_repair<1>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups)
-     : mx ? batch_shape(ctx, k_dijkstra_batch<1, true>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups)
-          : batch_shape(ctx, k_dijkstra_batch<1>, n, per_group, ctx->dws_groups, "Dijkstra", &cs, &groups);
-  if (rc != MNB_OK) return rc;
-  if (groups > ctx->dws_groups) {
-    ctx->dws = DijkstraBatchBuffers{};        // the smaller workspace goes first: batch_shape has counted its bytes as available
-    ctx->dws_groups = 0; ctx->dws_marks_clean = false;
-    const size_t m = (size_t)groups * V;
-    CK(ctx->dws.label.reserve(m)); CK(ctx->dws.mark.reserve(m)); CK(ctx->dws.list0.reserve(m)); CK(ctx->dws.list1.reserve(m));
-    CK(ctx->dws.ctl.reserve(groups));
-    ctx->dws_groups = groups;
-  }
-  if (ctx->h_cancel) *ctx->h_cancel = 0;     // dijkstra:238
-  if ((rc = ensure_adj_tables(ctx)) != MNB_OK) return rc;
-  CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_vertices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
-  CK(cudaMemsetAsync(ctx->dws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+  CallerArrays io(ctx);      // host-pointer staging, reserved before the workspace is sized
+  float* const o_matrix = mx ? io.out(mx->out, ctx->d_out_dist, (size_t)n * mx->m) : nullptr;
+  float* const o_dist = rq ? io.inout(out_dist, ctx->d_out_dist, rows) : io.out(out_dist, ctx->d_out_dist, rows);
+  uint32_t* const o_pred = rq ? io.inout(out_pred, ctx->d_batch_pred, rows) : io.out(out_pred, ctx->d_batch_pred, rows);
+  CK(io.status());
   DijkstraBatchArgs a{};
-  a.V = ctx->V; a.adj_ptr = ctx->d_adj_ptr; a.adj_nw = ctx->d_adj_nw; a.cost = ctx->d_cost;
-  a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = dijkstra_workspace(ctx);
-  a.n_queries = n; a.seeds = ctx->d_seed_faces; a.cost_limit = cost_limit; a.delta = ctx->dijkstra_batch_delta;
-  a.out_dist = !out_dist ? nullptr : (dev ? out_dist : ctx->d_out_dist);
-  a.out_pred = !out_pred ? nullptr : (dev ? out_pred : ctx->d_batch_pred);
-  a.next_query = ctx->d_next_query; a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V);
-  if (mx) {
-    if ((rc = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return rc;
-    a.tg.out = dev ? mx->out : ctx->d_out_dist;
-  }
   DijkstraRepairArgs ra{};
-  if (rq) {
-    static_cast<DijkstraBatchArgs&>(ra) = a;
-    if ((rc = upload_changed(ctx, *rq, groups, ra.chg)) != MNB_OK) return rc;
-    // the repair resets the marks it sets; the batch kernel leaves its marks behind, a new workspace holds anything
-    if (!ctx->dws_marks_clean) CK(cudaMemsetAsync(ctx->dws.mark, 0, sizeof(uint32_t) * (size_t)ctx->dws_groups * V, ctx->stream));
-    if (!dev) {
-      CK(cudaMemcpyAsync(a.out_dist, out_dist, sizeof(float) * (size_t)n * V, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaMemcpyAsync(a.out_pred, out_pred, sizeof(uint32_t) * (size_t)n * V, cudaMemcpyHostToDevice, ctx->stream));
+  auto prepare = [&](unsigned groups) -> int32_t {
+    int32_t r;
+    if ((r = ensure_dijkstra_workspace(ctx, groups)) != MNB_OK) return r;
+    if (ctx->h_cancel) *ctx->h_cancel = 0;     // dijkstra:238
+    if ((r = ensure_adj_tables(ctx)) != MNB_OK) return r;
+    CK(cudaMemcpyAsync(ctx->d_seed_faces, seed_vertices, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
+    CK(cudaMemsetAsync(ctx->dws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+    a.V = ctx->V; a.adj_ptr = ctx->d_adj_ptr; a.adj_nw = ctx->d_adj_nw; a.cost = ctx->d_cost;
+    a.invalid = ctx->has_invalid ? ctx->d_invalid.p : nullptr; a.ws = dijkstra_workspace(ctx);
+    a.n_queries = n; a.seeds = ctx->d_seed_faces; a.cost_limit = cost_limit; a.delta = ctx->dijkstra_batch_delta;
+    a.out_dist = o_dist; a.out_pred = o_pred;
+    a.next_query = ctx->d_next_query; a.cancel_flag = ctx->d_cancel; a.max_rounds = watchdog_rounds(ctx->V);
+    if (mx) {
+      if ((r = upload_targets(ctx, *mx, a.tg)) != MNB_OK) return r;
+      a.tg.out = o_matrix;
     }
-  }
-  ctx->dws_marks_clean = false;
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  const unsigned blocks = groups * (unsigned)cs;
-  const cudaError_t e = with_cluster_size<8>(cs, [&](auto c) {
-    constexpr int CS = decltype(c)::value;
-    return rq ? launch_cluster(k_dijkstra_batch_repair<CS>, ra, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
-         : mx ? launch_cluster(k_dijkstra_batch<CS, true>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream)
-              : launch_cluster(k_dijkstra_batch<CS>, a, CS, blocks, MNB_BATCH_THREADS, ctx->stream);
-  });
-  if (e != cudaSuccess) { ctx->err = std::string("dijkstra batch launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
-  CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if ((rc = copy_matrix_out(ctx, n, mx)) != MNB_OK) return rc;
-  if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, a.out_dist, sizeof(float) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_pred) CK(cudaMemcpyAsync(out_pred, a.out_pred, sizeof(uint32_t) * (size_t)n * V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+    if (rq) {
+      static_cast<DijkstraBatchArgs&>(ra) = a;
+      if ((r = upload_changed(ctx, *rq, groups, ra.chg)) != MNB_OK) return r;
+      // the repair resets the marks it sets; the batch kernel leaves its marks behind, a new workspace holds anything
+      if (!ctx->dws_marks_clean) CK(cudaMemsetAsync(ctx->dws.mark, 0, sizeof(uint32_t) * (size_t)ctx->dws_groups * V, ctx->stream));
+    }
+    ctx->dws_marks_clean = false;
+    return MNB_OK;
+  };
+  const size_t per_group = DIJKSTRA_BATCH_BYTES_PER_VERTEX * V + sizeof(GroupCtl);
+  unsigned groups = 1;
+  rc = rq ? run_batch(ctx, [](auto c) { return k_dijkstra_batch_repair<decltype(c)::value>; }, ra, n, per_group, ctx->dws_groups, "Dijkstra", prepare, &groups)
+     : mx ? run_batch(ctx, [](auto c) { return k_dijkstra_batch<decltype(c)::value, true>; }, a, n, per_group, ctx->dws_groups, "Dijkstra", prepare, &groups)
+          : run_batch(ctx, [](auto c) { return k_dijkstra_batch<decltype(c)::value>; }, a, n, per_group, ctx->dws_groups, "Dijkstra", prepare, &groups);
+  if (rc != MNB_OK) return rc;
+  CK(io.copy_back());
   if ((rc = finish_stats(ctx, groups, 1, ctx->dws.ctl)) != MNB_OK) return rc;
   ctx->dws_marks_clean = rq != nullptr;      // every wave of the repair has reset its marks (a canceled one too)
   if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
@@ -1069,7 +1107,7 @@ static int32_t impl_dijkstra_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* see
 int32_t mnb_get_vertex_normals(mnb_ctx* ctx, float* out) {
   if (!ctx || !out || !ctx->V) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
-  CK(cudaMemcpyAsync(out, ctx->d_vertex_normals, sizeof(float) * 3 * (size_t)ctx->V, out_kind(ctx), ctx->stream));
+  CK(CallerArrays(ctx).copy_out(out, ctx->d_vertex_normals.p, 3 * (size_t)ctx->V));
   CK(cudaStreamSynchronize(ctx->stream));
   return MNB_OK;
 }
@@ -1081,18 +1119,18 @@ static int32_t impl_compute_layers(mnb_ctx* ctx, const mnb_layer_params* params,
   const size_t V = ctx->V;
   CK(ctx->d_layer_costs.reserve(6 * V)); CK(ctx->d_layer_combined.reserve(V)); CK(ctx->d_layer_mask.reserve(V));
   CK(ctx->d_overflow.reserve(1));
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  if (clearance) {
-    CK(ctx->d_clearance.reserve(V));
-    CK(cudaMemcpyAsync(ctx->d_clearance, clearance, sizeof(float) * V, in_kind(ctx), ctx->stream));
-  }
+  if (clearance) CK(ctx->d_clearance.reserve(V));
+  CallerArrays io(ctx);
+  const float* const d_clear = io.in(clearance, ctx->d_clearance.p, V);
+  float* const o_costs = io.needed(out_costs, ctx->d_layer_costs.p, 6 * V);
+  float* const o_combined = io.needed(out_combined, ctx->d_layer_combined.p, V);
+  uint8_t* const o_mask = io.needed(out_lethal_mask, ctx->d_layer_mask.p, V);
+  CK(io.status());
   CK(cudaMemsetAsync(ctx->d_overflow, 0, sizeof(unsigned int), ctx->stream));
   LayerKernelArgs a{};
   a.V = ctx->V; a.pos = ctx->d_pos; a.vn = ctx->d_vertex_normals; a.adj_ptr = ctx->d_adj_ptr; a.adj_nbr = ctx->d_adj_nbr;
-  a.border = ctx->d_border; a.clearance = clearance ? ctx->d_clearance.p : nullptr; a.P = *params;
-  a.costs = (dev && out_costs) ? out_costs : ctx->d_layer_costs;
-  a.combined = (dev && out_combined) ? out_combined : ctx->d_layer_combined;
-  a.lethal_mask = (dev && out_lethal_mask) ? out_lethal_mask : ctx->d_layer_mask;
+  a.border = ctx->d_border; a.clearance = d_clear; a.P = *params;
+  a.costs = o_costs; a.combined = o_combined; a.lethal_mask = o_mask;
   a.overflow = ctx->d_overflow;
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   if (ctx->layers_smem) {
@@ -1132,11 +1170,7 @@ static int32_t impl_compute_layers(mnb_ctx* ctx, const mnb_layer_params* params,
   }
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    if (out_costs) CK(cudaMemcpyAsync(out_costs, a.costs, sizeof(float) * 6 * V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_combined) CK(cudaMemcpyAsync(out_combined, a.combined, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_lethal_mask) CK(cudaMemcpyAsync(out_lethal_mask, a.lethal_mask, V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   unsigned int ovf = 0;
   CK(cudaMemcpyAsync(&ovf, ctx->d_overflow, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
@@ -1150,24 +1184,19 @@ static int32_t impl_vector_map(mnb_ctx* ctx, const uint32_t* pred, const float* 
   if (!pred && !ctx->last_valid) { ctx->err = "mnb_vector_map(pred = NULL) needs a successful mnb_cvp on this context first"; return MNB_E_STATE; }
   CK(cudaSetDevice(ctx->device));
   const size_t V = ctx->V;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  const uint32_t* d_pred = pred; const float* d_dir = direction; const int32_t* d_cut = cutting_face; float* d_out = out_vec;
+  CallerArrays io(ctx);
   DeviceBuffer<float> tmp_out, tmp_dir; DeviceBuffer<uint32_t> tmp_pred; DeviceBuffer<int32_t> tmp_cut;
-  if (!pred) {            // the device-resident result of the last CVP plan (nothing is uploaded)
-    d_pred = ctx->last_pred; d_dir = ctx->last_dir; d_cut = ctx->last_cut;
-    if (!dev) { CK(tmp_out.reserve(3 * V)); d_out = tmp_out; }
-  } else if (!dev) {
-    CK(tmp_out.reserve(3 * V)); CK(tmp_pred.reserve(V));
-    CK(cudaMemcpyAsync(tmp_pred, pred, sizeof(uint32_t) * V, cudaMemcpyHostToDevice, ctx->stream));
-    d_pred = tmp_pred; d_out = tmp_out;
-    if (direction) { CK(tmp_dir.reserve(V)); CK(cudaMemcpyAsync(tmp_dir, direction, sizeof(float) * V, cudaMemcpyHostToDevice, ctx->stream)); d_dir = tmp_dir; }
-    if (cutting_face) { CK(tmp_cut.reserve(V)); CK(cudaMemcpyAsync(tmp_cut, cutting_face, sizeof(int32_t) * V, cudaMemcpyHostToDevice, ctx->stream)); d_cut = tmp_cut; }
-  }
+  float* const d_out = io.out(out_vec, tmp_out, 3 * V);
+  // pred NULL: the device-resident result of the last CVP plan (nothing is uploaded)
+  const uint32_t* const d_pred = pred ? io.in(pred, tmp_pred, V) : ctx->last_pred;
+  const float* const d_dir = pred ? io.in(direction, tmp_dir, V) : ctx->last_dir;
+  const int32_t* const d_cut = pred ? io.in(cutting_face, tmp_cut, V) : ctx->last_cut;
+  CK(io.status());
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   MNB_LAUNCH(k_vector_map, (ctx->V + 255) / 256, 256, 0, ctx->stream, ctx->d_pos, ctx->d_vertex_normals, d_pred, d_dir, d_cut, ctx->V, d_out);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) CK(cudaMemcpyAsync(out_vec, d_out, sizeof(float) * 3 * V, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(io.copy_back());
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, 1, ctx->V);
   return MNB_OK;
@@ -1181,12 +1210,14 @@ static int32_t impl_cvp_backtrack(mnb_ctx* ctx, const float robot_pos[3], uint32
   CK(cudaSetDevice(ctx->device));
   CK(ctx->d_path_pos.reserve(3 * (size_t)max_points)); CK(ctx->d_path_face.reserve(max_points));
   CK(ctx->d_bt_result.reserve(2));
+  uint32_t n = 0;           // points written: read back after the launch
+  CallerArrays io(ctx);
   BacktrackArgs a{};
   a.pos = ctx->d_pos; a.vn = ctx->d_vertex_normals; a.faces = ctx->d_faces; a.cor_ptr = ctx->d_cor_ptr; a.cor_idx = ctx->d_cor_idx;
   a.pred = ctx->last_pred; a.direction = ctx->last_dir; a.cut = ctx->last_cut;
   for (int k = 0; k < 3; ++k) { a.start[k] = ctx->last_seed_pos[k]; a.goal[k] = robot_pos[k]; }
   a.start_face = ctx->last_seed_face; a.goal_face = robot_face; a.step_width = step_width; a.max_points = max_points;
-  a.path_pos = ctx->d_path_pos; a.path_face = ctx->d_path_face; a.result = ctx->d_bt_result; a.cancel_flag = ctx->d_cancel;
+  a.path_pos = io.out(path_pos, ctx->d_path_pos.p, 3, &n); a.path_face = io.needed(path_face, ctx->d_path_face.p, 1, &n); a.result = ctx->d_bt_result; a.cancel_flag = ctx->d_cancel;
   a.layer = RepulsiveField{};
   if (ctx->repulsive_on && ctx->infl_field_valid) a.layer = repulsive_field_of(ctx);
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
@@ -1197,11 +1228,9 @@ static int32_t impl_cvp_backtrack(mnb_ctx* ctx, const float robot_pos[3], uint32
   int32_t res[2] = {0, 0};
   CK(cudaMemcpyAsync(res, ctx->d_bt_result, sizeof(res), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  const uint32_t n = (uint32_t)res[1] < max_points ? (uint32_t)res[1] : max_points;
+  n = (uint32_t)res[1] < max_points ? (uint32_t)res[1] : max_points;
   *n_points = n;
-  const cudaMemcpyKind kind = ctx->ptr_mode == MNB_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  CK(cudaMemcpyAsync(path_pos, ctx->d_path_pos, sizeof(float) * 3 * (size_t)n, kind, ctx->stream));
-  if (path_face) CK(cudaMemcpyAsync(path_face, ctx->d_path_face, sizeof(uint32_t) * (size_t)n, kind, ctx->stream));
+  CK(io.copy_back());
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, 1, n);
   if (res[0] == MNB_E_STATE) { ctx->err = "back-tracking exceeded max_points (cyclic vector field?) or the face search list"; return MNB_E_STATE; }
@@ -1211,16 +1240,15 @@ static int32_t impl_cvp_backtrack(mnb_ctx* ctx, const float robot_pos[3], uint32
 static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32_t* out_vertex, int32_t* out_face, float* out_bary) {
   if (!ctx || !ctx->V || !points || n == 0) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   DeviceBuffer<float> d_pts, d_b; DeviceBuffer<unsigned long long> d_keys; DeviceBuffer<uint32_t> d_v; DeviceBuffer<int32_t> d_f;
   CK(d_keys.reserve((size_t)n));
   CK(cudaMemsetAsync(d_keys, 0xff, sizeof(unsigned long long) * (size_t)n, ctx->stream));
-  const float* pts = points;
-  if (!dev) {
-    CK(d_pts.reserve(3 * (size_t)n)); CK(d_v.reserve((size_t)n)); CK(d_f.reserve((size_t)n)); CK(d_b.reserve(3 * (size_t)n));
-    CK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-    pts = d_pts;
-  }
+  CallerArrays io(ctx);
+  const float* const pts = io.in(points, d_pts, 3 * (size_t)n);
+  uint32_t* const o_vertex = io.out(out_vertex, d_v, n);
+  int32_t* const o_face = io.out(out_face, d_f, n);
+  float* const o_bary = io.out(out_bary, d_b, 3 * (size_t)n);
+  CK(io.status());
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   const uint32_t want = (ctx->V + 255) / 256, cap = (uint32_t)ctx->sm_count * 8;
   const uint32_t blocks = want < cap ? want : cap;
@@ -1228,14 +1256,10 @@ static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32
   for (uint32_t q0 = 0; q0 < n; q0 += LOC_Q, ++launches)
     MNB_LAUNCH(k_nearest_vertex, blocks, 256, 0, ctx->stream, ctx->d_pos, ctx->V, pts, q0, n - q0 < (uint32_t)LOC_Q ? n - q0 : (uint32_t)LOC_Q, d_keys);
   MNB_LAUNCH(k_containing_face, (n + 127) / 128, 128, 0, ctx->stream, ctx->d_pos, ctx->d_faces, ctx->d_cor_ptr, ctx->d_cor_idx, pts, n, d_keys,
-                                                           dev ? out_vertex : d_v, dev ? out_face : d_f, dev ? out_bary : d_b);
+             o_vertex, o_face, o_bary);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    if (out_vertex) CK(cudaMemcpyAsync(out_vertex, d_v, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_face) CK(cudaMemcpyAsync(out_face, d_f, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_bary) CK(cudaMemcpyAsync(out_bary, d_b, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, launches + 1, n);
   return MNB_OK;
@@ -1274,11 +1298,12 @@ static int32_t stage_inflation(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n
   if ((rc = ensure_workspace(ctx, 1)) != MNB_OK) return rc;
   if ((rc = ensure_out(ctx, (size_t)ctx->V, false)) != MNB_OK) return rc;
   CK(ctx->d_out_cost.reserve(ctx->V));
+  CallerArrays io(ctx);
   CK(d_lethals.reserve(n));
-  if (n) CK(cudaMemcpyAsync(d_lethals, lethals, sizeof(uint32_t) * n, in_kind(ctx), ctx->stream));
+  if (n) CK(io.copy_in(d_lethals.p, lethals, n));
   if (invalid) {
     CK(d_invalid.reserve(ctx->V));
-    CK(cudaMemcpyAsync(d_invalid, invalid, (size_t)ctx->V, in_kind(ctx), ctx->stream));
+    CK(io.copy_in(d_invalid.p, invalid, ctx->V));
   }
   return MNB_OK;
 }
@@ -1316,15 +1341,13 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
   ctx->infl_resident = false; ctx->infl_cid_valid = false; ctx->infl_field_resident = false;
   int32_t rc;
   if ((rc = stage_inflation(ctx, lethals, n, invalid, ctx->d_lethals, ctx->d_infl_invalid)) != MNB_OK) return rc;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  float* const o_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist.p;
-  float* const o_cost = (dev && out_cost) ? out_cost : ctx->d_out_cost.p;
+  // both outputs are produced without the caller's arrays too: they become the resident distances and riskiness
+  CallerArrays io(ctx);
+  float* const o_dist = io.needed(out_dist, ctx->d_out_dist.p, ctx->V);
+  float* const o_cost = io.needed(out_cost, ctx->d_out_cost.p, ctx->V);
   if ((rc = launch_inflate(ctx, ctx->d_lethals, n, invalid ? ctx->d_infl_invalid.p : nullptr, params, o_dist, o_cost, true)) != MNB_OK) return rc;
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, o_dist, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_cost) CK(cudaMemcpyAsync(out_cost, o_cost, sizeof(float) * (size_t)ctx->V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   int32_t rc2 = finish_stats(ctx, 1, 1);
   if (rc2 != MNB_OK) return rc2;
   // the riskiness map of this run is the "previous" one of the next mnb_inflation_update (riskiness_ = std::move(new_costs))
@@ -1333,16 +1356,16 @@ static int32_t inflate_impl(mnb_ctx* ctx, const uint32_t* lethals, uint32_t n, c
     const uint32_t n_tiles = (uint32_t)((V + US_TILE - 1) / US_TILE);
     CK(ctx->d_changed.reserve(V)); CK(ctx->d_tile_count.reserve(n_tiles)); CK(ctx->d_total.reserve(1));
     const float* old = ctx->prev_risk_valid ? ctx->d_prev_risk.p : nullptr;
-    uint32_t* d_out = (dev && out_changed) ? out_changed : ctx->d_changed;
+    unsigned int total = 0;
+    uint32_t* const d_out = io.needed(out_changed, ctx->d_changed.p, 1, &total);
     MNB_LAUNCH(k_update_set_count, n_tiles, 256, 0, ctx->stream, (const float*)o_cost, old, ctx->V, ctx->d_tile_count);
     MNB_LAUNCH(k_update_set_scan, 1, 1024, 0, ctx->stream, ctx->d_tile_count, n_tiles, ctx->d_total);
     MNB_LAUNCH(k_update_set_write, n_tiles, 256, 0, ctx->stream, (const float*)o_cost, old, ctx->V, (const unsigned int*)ctx->d_tile_count, d_out);
     CK(cudaGetLastError());
-    unsigned int total = 0;
     CK(cudaMemcpyAsync(&total, ctx->d_total, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (n_changed) *n_changed = total;
-    if (!dev && out_changed && total) CK(cudaMemcpyAsync(out_changed, d_out, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(io.copy_back());
     ctx->stats.kernel_launches += 3;
   }
   CK(ctx->d_prev_risk.reserve(V));
@@ -1366,7 +1389,6 @@ static int32_t impl_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint
   if (!ctx || !ctx->V || !params || (n && !lethals) || !n_changed) return MNB_E_ARG;
   CK(cudaSetDevice(ctx->device));
   const uint32_t V = ctx->V, W = V / 32 + 1;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   const bool local = ctx->infl_resident && std::memcmp(params, &ctx->infl_params, sizeof(mnb_inflation_params)) == 0;
   const bool field = ctx->infl_field_valid, has_risk = ctx->prev_risk_valid, labels = ctx->infl_labels_valid;
   ctx->infl_labels_valid = false;
@@ -1383,8 +1405,12 @@ static int32_t impl_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint
   uint32_t* const aff = old_bits + 2 * (size_t)W; uint32_t* const chg = old_bits + 3 * (size_t)W;
   unsigned int* const d_cnt = ctx->d_infl_cnt;
   const uint8_t* const new_inv = invalid ? ctx->d_infl_invalid_next.p : nullptr;
-  float* const o_dist = (dev && out_dist) ? out_dist : ctx->d_out_dist.p;
-  float* const o_cost = (dev && out_cost) ? out_cost : ctx->d_out_cost.p;
+  // the changed list, then the dense outputs of a wave: without a wave the outputs are copies of the resident arrays
+  unsigned int total = 0;
+  CallerArrays list(ctx), rows(ctx);
+  uint32_t* const d_out = list.needed(out_changed, ctx->d_changed.p, 1, &total);
+  float* const o_dist = rows.needed(out_dist, ctx->d_out_dist.p, V);
+  float* const o_cost = rows.needed(out_cost, ctx->d_out_cost.p, V);
   CK(cudaMemsetAsync(old_bits, 0, sizeof(uint32_t) * 4 * (size_t)W, ctx->stream));
   CK(cudaMemsetAsync(d_cnt, 0, 6 * sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
@@ -1464,7 +1490,6 @@ static int32_t impl_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint
     ctx->infl_cid_valid = true;
   }
   // the changed set: ordered compaction of the bits the patch set
-  uint32_t* const d_out = (dev && out_changed) ? out_changed : ctx->d_changed.p;
   MNB_LAUNCH(k_bits_count, n_tiles, 256, 0, ctx->stream, (const uint32_t*)chg, W, ctx->d_tile_count);
   MNB_LAUNCH(k_update_set_scan, 1, 1024, 0, ctx->stream, ctx->d_tile_count, n_tiles, ctx->d_total);
   MNB_LAUNCH(k_bits_write, n_tiles, 256, 0, ctx->stream, (const uint32_t*)chg, W, (const unsigned int*)ctx->d_tile_count, d_out);
@@ -1483,15 +1508,16 @@ static int32_t impl_inflation_repair(mnb_ctx* ctx, const uint32_t* lethals, uint
     launches += fl;
   }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  unsigned int total = 0;
   CK(cudaMemcpyAsync(&total, ctx->d_total, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   *n_changed = total;
-  if (!dev && out_changed && total) CK(cudaMemcpyAsync(out_changed, d_out, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
-  const float* src_dist = ran ? o_dist : ctx->d_infl_dist.p;
-  const float* src_cost = ran ? o_cost : ctx->d_prev_risk.p;
-  if (out_dist && out_dist != src_dist) CK(cudaMemcpyAsync(out_dist, src_dist, sizeof(float) * (size_t)V, out_kind(ctx), ctx->stream));
-  if (out_cost && out_cost != src_cost) CK(cudaMemcpyAsync(out_cost, src_cost, sizeof(float) * (size_t)V, out_kind(ctx), ctx->stream));
+  CK(list.copy_back());
+  if (ran) {
+    CK(rows.copy_back());
+  } else {
+    if (out_dist) CK(rows.copy_out(out_dist, ctx->d_infl_dist.p, V));
+    if (out_cost) CK(rows.copy_out(out_cost, ctx->d_prev_risk.p, V));
+  }
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
   ctx->stats = mnb_stats{};
@@ -1520,8 +1546,9 @@ int32_t mnb_get_costs(mnb_ctx* ctx, float* out_vertex_costs, float* out_edge_wei
   if (!ctx || !ctx->V) return MNB_E_ARG;
   if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
   CK(cudaSetDevice(ctx->device));
-  if (out_vertex_costs) CK(cudaMemcpyAsync(out_vertex_costs, ctx->d_cost, sizeof(float) * (size_t)ctx->V, out_kind(ctx), ctx->stream));
-  if (out_edge_weights) CK(cudaMemcpyAsync(out_edge_weights, ctx->d_edge_w, sizeof(float) * (size_t)ctx->E, out_kind(ctx), ctx->stream));
+  CallerArrays io(ctx);
+  if (out_vertex_costs) CK(io.copy_out(out_vertex_costs, ctx->d_cost.p, ctx->V));
+  if (out_edge_weights) CK(io.copy_out(out_edge_weights, ctx->d_edge_w.p, ctx->E));
   CK(cudaStreamSynchronize(ctx->stream));
   return MNB_OK;
 }
@@ -1532,15 +1559,10 @@ static int32_t impl_update_vertex_costs(mnb_ctx* ctx, uint32_t n_changed, const 
   if (!ctx->costs_set) { ctx->err = "mnb_update_vertex_costs needs mnb_set_costs / mnb_compute_edge_weights first"; return MNB_E_STATE; }
   if (n_changed == 0) return MNB_OK;
   CK(cudaSetDevice(ctx->device));
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  const uint32_t* d_ids = changed; const float* d_costs = costs;
-  if (!dev) {
-    const size_t nc = costs_indexed_by_vertex ? (size_t)ctx->V : (size_t)n_changed;
-    CK(ctx->d_upd_ids.reserve(n_changed)); CK(ctx->d_upd_costs.reserve(nc));
-    CK(cudaMemcpyAsync(ctx->d_upd_ids, changed, sizeof(uint32_t) * (size_t)n_changed, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_upd_costs, costs, sizeof(float) * nc, cudaMemcpyHostToDevice, ctx->stream));
-    d_ids = ctx->d_upd_ids; d_costs = ctx->d_upd_costs;
-  }
+  CallerArrays io(ctx);
+  const uint32_t* const d_ids = io.in(changed, ctx->d_upd_ids, n_changed);
+  const float* const d_costs = io.in(costs, ctx->d_upd_costs, costs_indexed_by_vertex ? (size_t)ctx->V : (size_t)n_changed);
+  CK(io.status());
   if (!ctx->d_upd_stamp || ctx->upd_call == 0xffffffffu) {
     CK(ctx->d_upd_stamp.reserve(ctx->V));
     CK(cudaMemsetAsync(ctx->d_upd_stamp, 0, sizeof(uint32_t) * (size_t)ctx->V, ctx->stream));
@@ -1582,39 +1604,27 @@ static int32_t combination_update(mnb_ctx* ctx, uint32_t n_layers, const float* 
   for (uint32_t l = 0; l < n_layers; ++l) if (!layer_costs[l]) return MNB_E_ARG;
   if (n_changed == 0) return MNB_OK;
   CK(cudaSetDevice(ctx->device));
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
   const size_t V = ctx->V;
   CombineArgs a{};
   a.n_layers = n_layers; a.n = n_changed; a.V = ctx->V; a.average = weights ? 1 : 0;
   for (uint32_t l = 0; l < n_layers; ++l) a.weight[l] = weights ? weights[l] : 1.0f;
   // host-pointer mode: device copies of the maps, for this call
   DeviceBuffer<float> d_costs[COMB_MAX_LAYERS], d_io; DeviceBuffer<uint8_t> d_lethal[COMB_MAX_LAYERS], d_il; DeviceBuffer<uint32_t> d_ids;
-  auto up = [&](auto& buf, const auto* h, size_t n) -> cudaError_t {
-    const cudaError_t e = buf.reserve(n);
-    return e != cudaSuccess ? e : cudaMemcpyAsync(buf, h, sizeof(*h) * n, cudaMemcpyHostToDevice, ctx->stream);
-  };
+  CallerArrays io(ctx);
   for (uint32_t l = 0; l < n_layers; ++l) {
     a.def[l] = defaults[l];
-    if (dev) { a.costs[l] = layer_costs[l]; a.lethal[l] = layer_lethal ? layer_lethal[l] : nullptr; continue; }
-    CK(up(d_costs[l], layer_costs[l], V)); a.costs[l] = d_costs[l];
-    if (layer_lethal && layer_lethal[l]) { CK(up(d_lethal[l], layer_lethal[l], V)); a.lethal[l] = d_lethal[l]; }
+    a.costs[l] = io.in(layer_costs[l], d_costs[l], V);
+    a.lethal[l] = layer_lethal ? io.in(layer_lethal[l], d_lethal[l], V) : nullptr;
   }
-  if (!dev) {
-    CK(up(d_ids, changed, n_changed));
-    CK(up(d_io, io_costs, V));
-    if (io_lethal) CK(up(d_il, io_lethal, V));
-  }
-  a.changed = dev ? changed : d_ids;
-  a.io_costs = dev ? io_costs : d_io;
-  a.io_lethal = dev ? io_lethal : d_il;
+  a.changed = io.in(changed, d_ids, n_changed);
+  a.io_costs = io.inout(io_costs, d_io, V);
+  a.io_lethal = io.inout(io_lethal, d_il, V);
+  CK(io.status());
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   MNB_LAUNCH(k_max_combination_update, (n_changed + 255) / 256, 256, 0, ctx->stream, a);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    CK(cudaMemcpyAsync(io_costs, a.io_costs, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
-    if (io_lethal) CK(cudaMemcpyAsync(io_lethal, a.io_lethal, V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, 1, n_changed);
   return MNB_OK;

@@ -1,6 +1,6 @@
 // Host side of the ray caster (kernels_raycast.cuh): BVH build on first use, mnb_cast_rays, mnb_obstacle_update /
 // mnb_obstacle_reset, mnb_normal_clearance.  Included at the end of meshnav.cu (uses mnb_ctx and its RayCasterState, CK,
-// DeviceBuffer, simple_stats, the ordered compaction kernels of kernels_updates.cuh).
+// DeviceBuffer, CallerArrays, simple_stats, the ordered compaction kernels of kernels_updates.cuh).
 #pragma once
 #ifndef MNB_EMU_ACTIVE
 #include <cub/device/device_radix_sort.cuh>
@@ -101,33 +101,25 @@ static int32_t impl_cast_rays(mnb_ctx* ctx, uint32_t n, const float* origins, co
   if (rc != MNB_OK) return rc;
   ctx->stats = mnb_stats{};
   if (!n) return MNB_OK;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  CallerArrays io(ctx);
   const size_t nd = dir_stride ? 3 * (size_t)n : 3;
   // staging layout (floats): in = origins[3n] dirs[nd]; out = dist[n] face[n] point[3n] hit[n bytes]
-  if ((rc = ensure_ray_io(ctx, dev ? 0 : 3 * (size_t)n + nd, dev ? 0 : 6 * (size_t)n)) != MNB_OK) return rc;
-  const float* d_o = origins; const float* d_d = dirs;
-  float* d_dist = out_dist; uint32_t* d_face = out_face; float* d_point = out_point; uint8_t* d_hit = out_hit;
-  if (!dev) {
-    CK(cudaMemcpyAsync(ctx->d_ray_in, origins, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_ray_in + 3 * (size_t)n, dirs, sizeof(float) * nd, cudaMemcpyHostToDevice, ctx->stream));
-    d_o = ctx->d_ray_in; d_d = ctx->d_ray_in + 3 * (size_t)n;
-    d_dist = out_dist ? ctx->d_ray_out.p : nullptr;
-    d_face = out_face ? (uint32_t*)(ctx->d_ray_out + n) : nullptr;
-    d_point = out_point ? ctx->d_ray_out + 2 * (size_t)n : nullptr;
-    d_hit = out_hit ? (uint8_t*)(ctx->d_ray_out + 5 * (size_t)n) : nullptr;
-  }
+  if ((rc = ensure_ray_io(ctx, io.device() ? 0 : 3 * (size_t)n + nd, io.device() ? 0 : 6 * (size_t)n)) != MNB_OK) return rc;
+  float* const st_in = ctx->d_ray_in; float* const st_out = ctx->d_ray_out;
+  const float* const d_o = io.in(origins, st_in, 3 * (size_t)n);
+  const float* const d_d = io.in(dirs, st_in + 3 * (size_t)n, nd);
+  float* const d_dist = io.out(out_dist, st_out, n);
+  uint32_t* const d_face = io.out(out_face, (uint32_t*)(st_out + n), n);
+  float* const d_point = io.out(out_point, st_out + 2 * (size_t)n, 3 * (size_t)n);
+  uint8_t* const d_hit = io.out(out_hit, (uint8_t*)(st_out + 5 * (size_t)n), n);
+  CK(io.status());
   CK(cudaMemsetAsync(ctx->d_ray_overflow, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   MNB_LAUNCH(k_cast_rays, (n + 127) / 128, 128, 0, ctx->stream, ray_bvh(ctx), (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces, n,
              d_o, d_d, dir_stride, d_hit, d_dist, d_face, d_point, ctx->d_ray_overflow);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) {
-    if (out_dist) CK(cudaMemcpyAsync(out_dist, d_dist, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_face) CK(cudaMemcpyAsync(out_face, d_face, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_point) CK(cudaMemcpyAsync(out_point, d_point, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_hit) CK(cudaMemcpyAsync(out_hit, d_hit, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   if ((rc = check_ray_overflow(ctx)) != MNB_OK) return rc;
   simple_stats(ctx, 1, n);
   return MNB_OK;
@@ -149,7 +141,7 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
   int32_t rc = ensure_raycaster(ctx);
   if (rc != MNB_OK) return rc;
   const size_t V = ctx->V;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
+  CallerArrays io(ctx);
   const uint32_t n_tiles = (uint32_t)((V + US_TILE - 1) / US_TILE);
   if (!ctx->d_obst_mask) {
     CK(ctx->d_obst_now.reserve(V)); CK(ctx->d_obst_mask.reserve(V)); CK(ctx->d_obst_member.reserve(V));
@@ -157,19 +149,18 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
     CK(cudaMemsetAsync(ctx->d_obst_mask, 0, V, ctx->stream));
   }
   CK(ctx->d_changed.reserve(V)); CK(ctx->d_tile_count.reserve(n_tiles)); CK(ctx->d_total.reserve(1));
-  if ((rc = ensure_ray_io(ctx, dev ? 0 : 3 * (size_t)n_points, (!dev && out_costs) ? V : 0)) != MNB_OK) return rc;
-  const float* d_pts = points;
-  if (!dev && n_points) {
-    CK(cudaMemcpyAsync(ctx->d_ray_in, points, sizeof(float) * 3 * (size_t)n_points, cudaMemcpyHostToDevice, ctx->stream));
-    d_pts = ctx->d_ray_in;
-  }
+  if ((rc = ensure_ray_io(ctx, io.device() ? 0 : 3 * (size_t)n_points, (!io.device() && out_costs) ? V : 0)) != MNB_OK) return rc;
+  const float* const d_pts = n_points ? io.in(points, ctx->d_ray_in.p, 3 * (size_t)n_points) : points;
+  // the lists are produced without the caller's arrays too (the two halves of d_obst_list); their lengths are read back
+  unsigned int totals[2] = {0, 0};
+  uint32_t* const d_le = io.needed(out_lethals, ctx->d_obst_list.p, 1, &totals[0]);
+  uint32_t* const d_ch = io.needed(out_changed, ctx->d_obst_list + V, 1, &totals[1]);
+  float* const d_costs = io.out(out_costs, ctx->d_ray_out.p, V);
+  CK(io.status());
   ObstacleArgs a{};
   for (int k = 0; k < 12; ++k) a.tf[k] = P->tf[k];
   for (int k = 0; k < 3; ++k) a.axis[k] = P->down_axis[k];
   a.max_obstacle_dist = P->max_obstacle_dist; a.robot_height = P->robot_height;
-  float* d_costs = out_costs ? (dev ? out_costs : ctx->d_ray_out) : nullptr;
-  uint32_t* d_le = (dev && out_lethals) ? out_lethals : ctx->d_obst_list;
-  uint32_t* d_ch = (dev && out_changed) ? out_changed : ctx->d_obst_list + V;
   CK(cudaMemsetAsync(ctx->d_obst_now, 0, V, ctx->stream));
   CK(cudaMemsetAsync(ctx->d_ray_overflow, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
@@ -178,7 +169,6 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
                n_points, d_pts, a, ctx->d_obst_now, ctx->d_ray_overflow);
   MNB_LAUNCH(k_obstacle_diff, (unsigned)((V + 255) / 256), 256, 0, ctx->stream, ctx->V, (const uint8_t*)ctx->d_obst_now, ctx->d_obst_mask,
              ctx->d_obst_member, ctx->d_obst_member_chg, d_costs);
-  unsigned int totals[2] = {0, 0};
   for (int pass = 0; pass < 2; ++pass) {                   // ascending lists (std::set order): the new lethal set, the changed set
     const float* member = pass == 0 ? ctx->d_obst_member : ctx->d_obst_member_chg;
     MNB_LAUNCH(k_update_set_count, n_tiles, 256, 0, ctx->stream, member, (const float*)nullptr, ctx->V, ctx->d_tile_count);
@@ -191,11 +181,7 @@ static int32_t impl_obstacle_update(mnb_ctx* ctx, uint32_t n_points, const float
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   *n_lethals = totals[0]; *n_changed = totals[1];
-  if (!dev) {
-    if (out_lethals && totals[0]) CK(cudaMemcpyAsync(out_lethals, d_le, sizeof(uint32_t) * (size_t)totals[0], cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_changed && totals[1]) CK(cudaMemcpyAsync(out_changed, d_ch, sizeof(uint32_t) * (size_t)totals[1], cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_costs) CK(cudaMemcpyAsync(out_costs, d_costs, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  CK(io.copy_back());
   if ((rc = check_ray_overflow(ctx)) != MNB_OK) return rc;
   simple_stats(ctx, (n_points ? 1 : 0) + 7, n_points);
   return MNB_OK;
@@ -207,21 +193,18 @@ static int32_t impl_normal_clearance(mnb_ctx* ctx, const float* vertex_normals, 
   int32_t rc = ensure_raycaster(ctx);
   if (rc != MNB_OK) return rc;
   const size_t V = ctx->V;
-  const bool dev = ctx->ptr_mode == MNB_PTR_DEVICE;
-  if ((rc = ensure_ray_io(ctx, (!dev && vertex_normals) ? 3 * V : 0, dev ? 0 : V)) != MNB_OK) return rc;
-  const float* d_vn = ctx->d_vertex_normals;
-  if (vertex_normals) {
-    if (dev) d_vn = vertex_normals;
-    else { CK(cudaMemcpyAsync(ctx->d_ray_in, vertex_normals, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream)); d_vn = ctx->d_ray_in; }
-  }
-  float* d_out = dev ? out_clearance : ctx->d_ray_out;
+  CallerArrays io(ctx);
+  if ((rc = ensure_ray_io(ctx, (!io.device() && vertex_normals) ? 3 * V : 0, io.device() ? 0 : V)) != MNB_OK) return rc;
+  const float* const d_vn = vertex_normals ? io.in(vertex_normals, ctx->d_ray_in.p, 3 * V) : ctx->d_vertex_normals.p;
+  float* const d_out = io.out(out_clearance, ctx->d_ray_out.p, V);
+  CK(io.status());
   CK(cudaMemsetAsync(ctx->d_ray_overflow, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   MNB_LAUNCH(k_normal_clearance, (unsigned)((V + 127) / 128), 128, 0, ctx->stream, ray_bvh(ctx), (const float*)ctx->d_pos, (const uint32_t*)ctx->d_faces,
              ctx->V, d_vn, d_out, ctx->d_ray_overflow);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  if (!dev) CK(cudaMemcpyAsync(out_clearance, d_out, sizeof(float) * V, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(io.copy_back());
   if ((rc = check_ray_overflow(ctx)) != MNB_OK) return rc;
   simple_stats(ctx, 1, ctx->V);
   return MNB_OK;
