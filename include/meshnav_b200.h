@@ -118,6 +118,27 @@ int32_t mnb_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64
                 double cost_limit, double goal_dist_offset, float* out_dist, uint32_t* out_pred,
                 float* out_direction, int32_t* out_cutting_face);
 
+/* CVP replanning after cost updates: the outputs and the return code are bit-identical to mnb_cvp with the same
+ * arguments on the currently installed costs.  changed (n_changed entries, always a host pointer, any order, duplicates
+ * and unchanged vertices allowed) is the union of the changed sets of the mnb_update_vertex_costs calls since the last
+ * successful mnb_cvp_replan on this context; the caller keeps it, as for mnb_dijkstra_batch_repair.
+ * The context keeps the wave of the last successful replan in a workspace of its own (about 44 bytes per vertex plus the
+ * level pool, allocated by the first call).  When seed_face, the bits of seed_pos and of cost_limit are those of that
+ * wave and the costs changed since only through mnb_update_vertex_costs, the wave resumes from the earliest pop time the
+ * change can reach -- the earliest pop among the changed vertices and their face neighbours, the moment the old goal
+ * cutoff armed, or the moment the new robot face's vertices had all popped -- and re-runs only what comes after it;
+ * robot_face and goal_dist_offset may differ.  Otherwise (also after mnb_set_costs / mnb_compute_edge_weights / a cancelled
+ * call, when that moment is not after every seed's pop, or when the level pool lacks room) it runs one whole wave.
+ * mnb_get_stats counts the resumed part only (rounds, recomputes, settled).  mnb_cvp, the batch calls, the matrices,
+ * the field repair and the inflation calls may run between two replans without disturbing the resident wave.  On success
+ * the result is the last plan for mnb_cvp_backtrack and mnb_vector_map (pred = NULL), as after mnb_cvp.  Nothing is
+ * written on MNB_E_ARG (a changed id >= V, a NULL array that is needed), MNB_E_STATE (no costs), MNB_INVALID_START /
+ * MNB_INVALID_GOAL (as mnb_cvp).  mnb_cancel: MNB_CANCELED, and the next call runs a whole wave.  The outputs follow
+ * mnb_set_pointer_mode and may be NULL. */
+int32_t mnb_cvp_replan(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face,
+                       double cost_limit, double goal_dist_offset, uint32_t n_changed, const uint32_t* changed /* host */,
+                       float* out_dist, uint32_t* out_pred, float* out_direction, int32_t* out_cutting_face);
+
 /* Batched full-field CVP potentials: n independent goals on the installed map, one wavefront
  * per thread-block cluster, all SMs busy.  out_dist is [n][V] row-major.  Same call as mnb_cvp_batch_fields with
  * out_dist alone: the number of concurrent waves is capped by the free device memory as well. */

@@ -234,6 +234,16 @@ class MeshMap:
                                           _p(d_pred) if d_pred else None, _p(d_dir) if d_dir else None,
                                           _p(d_cut) if d_cut else None))
 
+    def cvp_replan_dev(self, seed_face, seed_pos, robot_face, cost_limit, goal_dist_offset, changed, d_dist: int,
+                       d_pred: int = 0, d_dir: int = 0, d_cut: int = 0) -> int:
+        """mnb_cvp_replan with device outputs (0 = not wanted); the changed vertices are host values"""
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32)
+        ch = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        opt = lambda d: _p(d) if d else None
+        return self._check(self.L.mnb_cvp_replan(self._ctx, int(seed_face), _p(sp), int(robot_face), float(cost_limit),
+                                                 float(goal_dist_offset), ch.size, _p(ch), opt(d_dist), opt(d_pred),
+                                                 opt(d_dir), opt(d_cut)))
+
     def cvp_batch_dev(self, seed_faces, seed_pos, cost_limit, d_out: int) -> int:
         sf = np.ascontiguousarray(seed_faces, dtype=np.uint32)
         sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
@@ -343,6 +353,24 @@ class CVPMeshPlanner:
         cut = out["cutting_face"] if out else np.empty(m.V, dtype=np.int32)
         rc = m._check(m.L.mnb_cvp(m._ctx, int(seed_face), _p(sp), int(robot_face), float(self.cost_limit),
                                   float(self.goal_dist_offset), _p(dist), _p(pred), _p(direction), _p(cut)))
+        return dict(outcome=rc, dist=dist, pred=pred, direction=direction, cutting_face=cut, **m.stats())
+
+    def waveFrontReplan(self, seed_face: int, seed_pos, robot_face: int = -1, changed=(), out=None):
+        """waveFrontPropagation after layerChanged calls whose changed vertices are `changed` (their union since the last
+        waveFrontReplan on this map): the same result, bit for bit.  When the seed face, seed position and cost limit
+        are those of the last replan and only layerChanged touched the costs since, the wave of that replan resumes from
+        the earliest moment the change can reach; otherwise one whole wave runs.  Returns what waveFrontPropagation
+        returns; `settled` counts the resumed part only."""
+        m = self.map
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32)
+        ch = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        dist = out["dist"] if out else np.empty(m.V, dtype=np.float32)
+        pred = out["pred"] if out else np.empty(m.V, dtype=np.uint32)
+        direction = out["direction"] if out else np.empty(m.V, dtype=np.float32)
+        cut = out["cutting_face"] if out else np.empty(m.V, dtype=np.int32)
+        rc = m._check(m.L.mnb_cvp_replan(m._ctx, int(seed_face), _p(sp), int(robot_face), float(self.cost_limit),
+                                         float(self.goal_dist_offset), ch.size, _p(ch), _p(dist), _p(pred), _p(direction),
+                                         _p(cut)))
         return dict(outcome=rc, dist=dist, pred=pred, direction=direction, cutting_face=cut, **m.stats())
 
     def computeVectorMap(self, pred, direction, cutting_face):

@@ -619,7 +619,9 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
 // Same round loop with 8 lanes per candidate (problem provides replay_sub8 / activate via its ELL row).
 // Used by the whole-grid single-plan kernel where per-round LATENCY is what matters.
 // -----------------------------------------------------------------------------
-template <int CS, bool SW, class P>
+// STOP_ON_OVERFLOW (the resumed replan wave): the loop also ends once the level pool has overflowed -- the host discards
+// the labels and runs the whole wave, so rounds on truncated pop times (which need not settle) would only cost time.
+template <int CS, bool SW, class P, bool STOP_ON_OVERFLOW = false>
 __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_t* list1, uint32_t* mark,
                                      Stage& st, const float delta, const uint32_t gthreads, const uint32_t gtid,
                                      const int has_robot, const uint32_t r0, const uint32_t r1, const uint32_t r2,
@@ -686,7 +688,8 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       ctl->m_tau[next] = INF_BITS;
       ctl->lo[next] = INF_BITS;
       atomicMin(&ctl->goal_ring[(r + 1) & 1], goal_b);                 // carry the cutoff into the next round
-      ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag)) ? 1u : 0u;
+      ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag) ||
+                                     (STOP_ON_OVERFLOW && __ldcg(&ctl->pool_overflow))) ? 1u : 0u;
     }
     // Goal cutoff (cvp:754 / dijkstra:299) with a band wider than goal_dist_offset: labels computed before the cutoff
     // is known may rest on sources that turn out to lie beyond it.  Once it is known, (1) vertices beyond it never

@@ -108,7 +108,9 @@ __device__ __forceinline__ void count_targets_done_at_init(const TargetSet& tg, 
 #ifndef MNB_CVP_THREADS
 #define MNB_CVP_THREADS 512
 #endif
-template <int CS>
+// RESUME (mnb_cvp_replan, single plan): the workspace holds a rolled-back wave (k_replan_rollback, k_replan_frontier), so
+// the clearing pass and the seeding are skipped and the band starts at T0 (DESIGN §4, "Replan").
+template <int CS, bool RESUME = false>
 __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(const CvpKernelArgs a) {
   __shared__ Stage st;
   uint32_t g, gthreads, gtid;
@@ -130,11 +132,13 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
     const bool single = (a.n_queries == 1);
     uint32_t* chg = a.ws.chg + (size_t)g * V;
     const int sweeps = 0;                            // in-round sweeps are compiled into the whole-grid kernel only
-    for (uint32_t v = gtid; v < V; v += gthreads) {
-      state[v] = state_inf(); mark[v] = MARK_NONE; chg[v] = 0u;
-      if (sweeps) a.ws.ver[v] = 0u;
+    if constexpr (!RESUME) {
+      for (uint32_t v = gtid; v < V; v += gthreads) {
+        state[v] = state_inf(); mark[v] = MARK_NONE; chg[v] = 0u;
+        if (sweeps) a.ws.ver[v] = 0u;
+      }
+      group_sync<CS>();
     }
-    group_sync<CS>();
 
     const uint32_t sf = a.seed_faces[q];
     const uint32_t s0 = a.faces[3 * (size_t)sf], s1 = a.faces[3 * (size_t)sf + 1], s2 = a.faces[3 * (size_t)sf + 2];
@@ -168,16 +172,18 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
     }
     if (gtid == 0) {
       const uint32_t sv[3] = {s0, s1, s2};
-      for (int k = 0; k < 3; ++k) {
-        state[sv[k]] = make_uint4(__float_as_uint(sd[k]), __float_as_uint(sd[k]), 0u, 0u);
-        mark[sv[k]] = MARK_FIXED;
+      if constexpr (!RESUME) {
+        for (int k = 0; k < 3; ++k) {
+          state[sv[k]] = make_uint4(__float_as_uint(sd[k]), __float_as_uint(sd[k]), 0u, 0u);
+          mark[sv[k]] = MARK_FIXED;
+        }
+        unsigned int n0 = 0;
+        for (int k = 0; k < 3; ++k)
+          prob.activate(sv[k], [&](uint32_t x) {
+            if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
+          });
+        ctl_reset(ctl, n0, seed_min);
       }
-      unsigned int n0 = 0;
-      for (int k = 0; k < 3; ++k)
-        prob.activate(sv[k], [&](uint32_t x) {
-          if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-        });
-      ctl_reset(ctl, n0, seed_min);
       if (has_robot) {
         int left = 0; const uint32_t rv[3] = {r0, r1, r2};
         for (int k = 0; k < 3; ++k) if (mark[rv[k]] != MARK_FIXED) left++;
@@ -193,8 +199,10 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
     group_sync<CS>();
     float delta = a.delta;
     if (has_robot && a.goal_dist_offset < (double)delta) delta = (float)fmax(a.goal_dist_offset, 1e-4);
-    run_band_rounds_sub8<CS, false>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, r0, r1, r2,
-                        a.goal_dist_offset, a.cancel_flag, nextafterf(seed_max, __uint_as_float(INF_BITS)), a.max_rounds, sweeps, nullptr, V);
+    // a resumed band starts at T0: every kept label (and seed) lies below it (k_replan_rollback set lo[2] = T0's key)
+    const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : seed_max;
+    run_band_rounds_sub8<CS, false, CvpEllProblem, RESUME>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, r0, r1, r2,
+                        a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)), a.max_rounds, sweeps, nullptr, V);
     group_sync<CS>();
     if (a.out_dist) {
       float* od = a.out_dist + (size_t)q * V;
@@ -361,6 +369,8 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
 #ifndef MNB_GRID_MINBLOCKS
 #define MNB_GRID_MINBLOCKS 1
 #endif
+// RESUME: as k_cvp<CS, true> (mnb_cvp_replan)
+template <bool RESUME = false>
 __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpKernelArgs a) {
   __shared__ Stage st;
   __shared__ SweepStage sws;
@@ -371,8 +381,10 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
   GroupCtl* ctl = a.ws.ctl;
   if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; sws.dn[0] = 0; sws.dn[1] = 0; }
   __syncthreads();
-  for (uint32_t v = gtid; v < V; v += gthreads) { state[v] = state_inf(); mark[v] = MARK_NONE; a.ws.chg[v] = 0u; a.ws.ver[v] = 0u; }
-  group_sync<0>(ctl->barrier);
+  if constexpr (!RESUME) {
+    for (uint32_t v = gtid; v < V; v += gthreads) { state[v] = state_inf(); mark[v] = MARK_NONE; a.ws.chg[v] = 0u; a.ws.ver[v] = 0u; }
+    group_sync<0>(ctl->barrier);
+  }
   const uint32_t sf = a.seed_faces[0];
   const uint32_t s0 = a.faces[3 * (size_t)sf], s1 = a.faces[3 * (size_t)sf + 1], s2 = a.faces[3 * (size_t)sf + 2];
   CvpEllProblem prob;
@@ -405,13 +417,15 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
   }
   if (gtid == 0) {
     const uint32_t sv[3] = {s0, s1, s2};
-    for (int k = 0; k < 3; ++k) { state[sv[k]] = make_uint4(__float_as_uint(sd[k]), __float_as_uint(sd[k]), 0u, 0u); mark[sv[k]] = MARK_FIXED; }
-    unsigned int n0 = 0;
-    for (int k = 0; k < 3; ++k)
-      prob.activate(sv[k], [&](uint32_t x) {
-        if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-      });
-    ctl_reset(ctl, n0, seed_min);
+    if constexpr (!RESUME) {
+      for (int k = 0; k < 3; ++k) { state[sv[k]] = make_uint4(__float_as_uint(sd[k]), __float_as_uint(sd[k]), 0u, 0u); mark[sv[k]] = MARK_FIXED; }
+      unsigned int n0 = 0;
+      for (int k = 0; k < 3; ++k)
+        prob.activate(sv[k], [&](uint32_t x) {
+          if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
+        });
+      ctl_reset(ctl, n0, seed_min);
+    }
     if (has_robot) {
       int left = 0; const uint32_t rv[3] = {r0, r1, r2};
       for (int k = 0; k < 3; ++k) if (mark[rv[k]] != MARK_FIXED) left++;
@@ -429,8 +443,9 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
   // in-round sweeps pay off once the band is several dependency hops deep; 12 were measured best on the 5M terrain
   int sweeps = a.sweeps;
   if (sweeps < 0) sweeps = delta < 2.8f * a.hop ? 0 : min(12, (int)(delta / a.hop));
-  run_band_rounds_sub8<0, true>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, r0, r1, r2,
-                          a.goal_dist_offset, a.cancel_flag, nextafterf(seed_max, __uint_as_float(INF_BITS)), a.max_rounds, sweeps, &sws, V);
+  const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : seed_max;    // (see k_cvp)
+  run_band_rounds_sub8<0, true, CvpEllProblem, RESUME>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, r0, r1, r2,
+                          a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)), a.max_rounds, sweeps, &sws, V);
   group_sync<0>(ctl->barrier);
   if (a.out_dist)
     for (uint32_t v = gtid; v < V; v += gthreads) a.out_dist[v] = __uint_as_float(state[v].x);
@@ -447,6 +462,179 @@ __global__ void __launch_bounds__(256) k_cvp_epilogue(const CvpKernelArgs a, Gro
   CvpProblem prob;
   cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, goal_t, a.out_pred, a.out_dir, a.out_cut, prob);
   cvp_epilogue_vertex(prob, ctl, sf, __uint_as_float(ctl->goal_bits), c);
+}
+
+// ============================================================================
+// CVP replan (mnb_cvp_replan): the resident single-plan wave resumes from the earliest pop time a cost change can reach
+// (DESIGN §4, "Replan").  Every event of the reference loop before
+//   T0 = min(pop times of the closed 1-rings of the changed vertices, the old wave's cutoff arming time,
+//            the latest old pop time of the new robot face's vertices)
+// reads only labels, gates and weights that did not change, so the vertices that popped before T0 keep their labels and
+// the rest of the wave is run again: k_replan_t0 + k_replan_t0_final reduce T0, k_replan_rollback keeps the prefix and
+// resets everything else, k_replan_frontier lists the first candidates, and k_cvp_grid<true> / k_cvp<CS, true> resume.
+// ============================================================================
+struct ReplanArgs {
+  uint32_t V;
+  const uint32_t* faces; const uint32_t* cor_ptr; const int4* cor_idx;
+  const float* cost; const uint8_t* invalid; double cost_limit;
+  WaveWorkspace ws;                 // the resident wave (one group)
+  const uint32_t* changed; uint32_t n_changed;   // device, any order, duplicates allowed
+  uint32_t seed_face;
+  long long robot_face;             // -1 = none
+  uint32_t* t0;                     // [8 + 6 * blocks of k_replan_t0]: T0, the resume flag, one spare word, the block minima
+};
+constexpr uint32_t REPLAN_T0_WORDS = 8;
+
+// a pop time as six words, in the order of GroupCtl::goal_time: a1 bits, root, a2 bits, a3 bits, ext, vertex
+__device__ __forceinline__ void time_put(uint32_t* w, const EvTime& t) {
+  w[0] = __float_as_uint(t.a1); w[1] = t.root; w[2] = __float_as_uint(t.a2); w[3] = __float_as_uint(t.a3); w[4] = t.ext; w[5] = t.self;
+}
+__device__ __forceinline__ EvTime time_get(const uint32_t* w) {
+  EvTime t; t.a1 = __uint_as_float(__ldcg(&w[0])); t.root = __ldcg(&w[1]); t.a2 = __uint_as_float(__ldcg(&w[2]));
+  t.a3 = __uint_as_float(__ldcg(&w[3])); t.ext = __ldcg(&w[4]); t.self = __ldcg(&w[5]);
+  return t;
+}
+// later than every finite pop time
+__device__ __forceinline__ EvTime time_never() { return ev_normal(__uint_as_float(INF_BITS), 0xffffffffu); }
+
+__device__ __forceinline__ LabelStore replan_store(const ReplanArgs& a) {
+  LabelStore s;
+  s.state = a.ws.state; s.root_arr = a.ws.root; s.ext_arr = a.ws.ext; s.chg = a.ws.chg;
+  s.pool = a.ws.pool; s.pool_w = a.ws.pool; s.pool_cap = a.ws.pool_cap; s.pool_top = &a.ws.ctl->pool_top; s.pool_overflow = &a.ws.ctl->pool_overflow;
+  return s;
+}
+
+// the earliest of the block's times t (every thread calls this; the result is valid in thread 0)
+__device__ __forceinline__ EvTime time_min_block(const TimeAlg& A, EvTime t) {
+  __shared__ uint32_t sw[32][6];
+  for (int o = 16; o > 0; o >>= 1) {
+    EvTime u;
+    u.a1 = __shfl_down_sync(0xffffffffu, t.a1, o); u.root = __shfl_down_sync(0xffffffffu, t.root, o);
+    u.a2 = __shfl_down_sync(0xffffffffu, t.a2, o); u.a3 = __shfl_down_sync(0xffffffffu, t.a3, o);
+    u.ext = __shfl_down_sync(0xffffffffu, t.ext, o); u.self = __shfl_down_sync(0xffffffffu, t.self, o);
+    if (A.tless(u, t)) t = u;
+  }
+  if ((threadIdx.x & 31) == 0) time_put(sw[threadIdx.x >> 5], t);
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (uint32_t w = 1; w < (blockDim.x + 31) / 32; ++w) {
+      EvTime u;                          // (plain loads: time_get reads global memory through the L2 only)
+      u.a1 = __uint_as_float(sw[w][0]); u.root = sw[w][1]; u.a2 = __uint_as_float(sw[w][2]); u.a3 = __uint_as_float(sw[w][3]);
+      u.ext = sw[w][4]; u.self = sw[w][5];
+      if (A.tless(u, t)) t = u;
+    }
+  return t;
+}
+
+// 1. per block: the earliest pop time over the changed vertices and their face neighbours (labels of the resident wave)
+__global__ void __launch_bounds__(256) k_replan_t0(const ReplanArgs a) {
+  const LabelStore S = replan_store(a);
+  EvTime best = time_never();
+  auto consider = [&](uint32_t x) {
+    const Label L = S.load_label(x);
+    if (__float_as_uint(L.d) != INF_BITS && S.tless(L.t, best)) best = L.t;
+  };
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n_changed; i += gridDim.x * blockDim.x) {
+    const uint32_t c = __ldg(&a.changed[i]);
+    consider(c);
+    for (uint32_t k = __ldg(&a.cor_ptr[c]), ke = __ldg(&a.cor_ptr[c + 1]); k < ke; ++k) {
+      const int4 ix = __ldg(&a.cor_idx[k]);
+      consider((uint32_t)ix.x); consider((uint32_t)ix.y);
+    }
+  }
+  best = time_min_block(S, best);
+  if (threadIdx.x == 0) time_put(a.t0 + REPLAN_T0_WORDS + 6 * blockIdx.x, best);
+}
+
+// 2. one block: T0 = min(block minima, the old cutoff's arming time, the new cutoff's arming time if the old wave knows
+//    it); t0[6] = 1 if every seed pops before T0 (otherwise the call runs a whole wave)
+__global__ void __launch_bounds__(256) k_replan_t0_final(const ReplanArgs a, uint32_t blocks) {
+  const LabelStore S = replan_store(a);
+  EvTime best = time_never();
+  for (uint32_t b = threadIdx.x; b < blocks; b += blockDim.x) {
+    const EvTime u = time_get(a.t0 + REPLAN_T0_WORDS + 6 * b);
+    if (S.tless(u, best)) best = u;
+  }
+  best = time_min_block(S, best);
+  if (threadIdx.x != 0) return;
+  // the old wave's goal cutoff: events after its arming differ with another robot face or offset (+inf key: not armed)
+  const EvTime armed = time_get(a.ws.ctl->goal_time);
+  if (__float_as_uint(armed.a1) != INF_BITS && S.tless(armed, best)) best = armed;
+  // the new goal cutoff arms when the last vertex of the robot face pops: if all three popped in the old wave before
+  // T0, that moment is the same in a fresh wave, and the events after it differ
+  if (a.robot_face >= 0) {
+    EvTime late = ev_normal(0.0f, 0u); bool all = true;
+    for (int k = 0; k < 3; ++k) {
+      const Label L = S.load_label(__ldg(&a.faces[3 * (size_t)a.robot_face + k]));
+      if (__float_as_uint(L.d) == INF_BITS) all = false;
+      else if (k == 0 || S.tless(late, L.t)) late = L.t;
+    }
+    if (all && S.tless(late, best)) best = late;
+  }
+  bool ok = true;
+  for (int k = 0; k < 3; ++k) ok = ok && S.tless(S.load_label(__ldg(&a.faces[3 * (size_t)a.seed_face + k])).t, best);
+  time_put(a.t0, best);
+  a.t0[6] = ok ? 1u : 0u;
+}
+
+// 3. the rollback: a vertex that popped before T0 (and every seed) stays settled with its label, pool record included;
+//    every other one gets the state of a fresh wave.  Vertices that can never be fixed (invalid, cost >= cost_limit) hold
+//    +inf and are reset with the rest.  The group's control block is reset for the round loop with the band at T0; the
+//    level pool keeps its records and allocation continues from its top.
+__global__ void __launch_bounds__(256) k_replan_rollback(const ReplanArgs a) {
+  const LabelStore S = replan_store(a);
+  const EvTime T0 = time_get(a.t0);
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v == 0) {
+    GroupCtl* ctl = a.ws.ctl;
+    const unsigned int top = ctl->pool_top;
+    *ctl = GroupCtl{};
+    ctl_reset(ctl, 0u, T0.a1);
+    ctl->pool_top = top;
+  }
+  if (v >= a.V) return;
+  const uint32_t* sv = a.faces + 3 * (size_t)a.seed_face;
+  const bool seed = v == __ldg(&sv[0]) || v == __ldg(&sv[1]) || v == __ldg(&sv[2]);
+  const Label L = S.load_label(v);
+  const bool keep = seed || (__float_as_uint(L.d) != INF_BITS && S.tless(L.t, T0));
+  if (keep) a.ws.mark[v] = MARK_FIXED;
+  else { a.ws.state[v] = state_inf(); a.ws.mark[v] = MARK_NONE; }
+  a.ws.chg[v] = 0u;
+  a.ws.ver[v] = 0u;
+}
+
+// 4. the first candidates: the vertices that may take a label (as k_cvp_grid's activation) and share a face with a kept
+//    vertex -- in a fresh wave the kept labels would have pulled them in
+__global__ void __launch_bounds__(256) k_replan_frontier(const ReplanArgs a) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= a.V) return;
+  uint32_t* mark = a.ws.mark;
+  const uint32_t mv = __ldcg(&mark[v]);
+#ifdef MNB_EMU_ACTIVE
+  // the interpreter checks two invariants of the rollback: the seeds stay fixed, and a kept label's level stack names
+  // only kept vertices (levels are running maxima of the pop sequence, so they popped before; LabelStore::names relies on it)
+  const uint32_t* sv = a.faces + 3 * (size_t)a.seed_face;
+  if ((v == sv[0] || v == sv[1] || v == sv[2]) && mv != MARK_FIXED) { fprintf(stderr, "[replan] seed %u not fixed\n", v); abort(); }
+  if (mv == MARK_FIXED) {
+    const LabelStore S = replan_store(a);
+    const Label L = S.load_label(v);
+    for (uint32_t i = 1, n = S.levels_of(L.t); i <= n; ++i) {
+      uint32_t kb, id; S.level_of(L.t, i, kb, id);
+      if (id != v && mark[id] != MARK_FIXED) { fprintf(stderr, "[replan] kept label of %u names reset vertex %u\n", v, id); abort(); }
+    }
+  }
+#endif
+  if (mv != MARK_NONE) return;
+  if ((a.invalid && a.invalid[v]) || (double)a.cost[v] >= a.cost_limit) return;
+  bool next_to_kept = false;
+  for (uint32_t k = __ldg(&a.cor_ptr[v]), ke = __ldg(&a.cor_ptr[v + 1]); k < ke && !next_to_kept; ++k) {
+    const int4 ix = __ldg(&a.cor_idx[k]);
+    next_to_kept = __ldcg(&mark[ix.x]) == MARK_FIXED || __ldcg(&mark[ix.y]) == MARK_FIXED;
+  }
+  if (next_to_kept) {
+    mark[v] = MARK_CAND;
+    a.ws.list0[atomicAdd(&a.ws.ctl->count[0], 1u)] = v;
+  }
 }
 
 // start == goal (dijkstra_mesh_planner.cpp:252-255): the maps as the reference leaves them after clearing (:241-249)

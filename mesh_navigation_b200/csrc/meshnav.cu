@@ -117,6 +117,15 @@ struct MeshState : RayCasterState {
   // device-resident result of the last single CVP plan (for mnb_cvp_backtrack)
   const uint32_t* last_pred = nullptr; const float* last_dir = nullptr; const int32_t* last_cut = nullptr;
   uint32_t last_seed_face = 0; float last_seed_pos[3] = {0, 0, 0}; bool last_valid = false;
+  // generation of the installed costs: mnb_set_costs and mnb_compute_edge_weights start a new one (mnb_set_mesh a new
+  // MeshState), mnb_update_vertex_costs does not -- a replan may resume across it
+  uint64_t cost_gen = 0;
+  // mnb_cvp_replan: the resident wave of the last successful replan in its own workspace (labels, side arrays, level pool,
+  // marks, lists, sweep versions, control block; allocated by the first replan) and what it was computed for
+  WaveBuffers rw;
+  bool rw_valid = false; uint32_t rw_seed_face = 0, rw_seed_pos[3] = {0, 0, 0}; uint64_t rw_cost_limit = 0, rw_cost_gen = 0;
+  uint32_t rw_pool_top = 0;
+  DeviceBuffer<uint32_t> d_replan_chg, d_replan_t0;      // the changed list of a replan, T0 and the block minima of its reduction
   DeviceBuffer<float> d_path_pos; DeviceBuffer<uint32_t> d_path_face; DeviceBuffer<int32_t> d_bt_result;
   DeviceBuffer<uint8_t> d_infl_invalid;
   // repulsive vector field of the last inflation (InflationLayer::vector_map_ / distances_)
@@ -160,6 +169,7 @@ struct mnb_ctx : MeshState {
                                // threads per CTA), 5-7 the same with the 16-bit seen-set (64 / 128 / 256), 8-9 its low-register builds.
                                // Chosen per mesh by mnb_set_mesh unless fixed by mnb_debug_set_layers_smem.
   bool layers_explicit = false;
+  uint32_t replan_pool_room = 0;   // level-pool words a resumed replan wave may add (mnb_debug_set_replan_pool_room; 0 = the pool's)
   int sweeps = -1;             // in-round sweeps of the whole-grid single plans (mnb_debug_set_sweeps); -1 = derived from the band width
   float grid_delta = 1.8f;     // band width of the whole-grid single-plan kernel (wide band + in-round sweeps)
   float dijkstra_grid_delta = 3.0f;
@@ -527,6 +537,7 @@ static int32_t ensure_adj_tables(mnb_ctx* ctx) {
 
 static int32_t impl_compute_edge_weights(mnb_ctx* ctx, const float* vertex_costs, double edge_cost_factor, float* out_w) {
   if (!ctx || !vertex_costs || !ctx->V) return MNB_E_ARG;
+  ++ctx->cost_gen;
   CK(cudaSetDevice(ctx->device));
   CallerArrays io(ctx);
   CK(io.copy_in(ctx->d_cost.p, vertex_costs, ctx->V));
@@ -541,6 +552,7 @@ static int32_t impl_compute_edge_weights(mnb_ctx* ctx, const float* vertex_costs
 
 static int32_t impl_set_costs(mnb_ctx* ctx, const float* vertex_costs, const float* edge_weights, const uint8_t* invalid) {
   if (!ctx || !vertex_costs || !edge_weights || !ctx->V) return MNB_E_ARG;
+  ++ctx->cost_gen;
   CK(cudaSetDevice(ctx->device));
   CallerArrays io(ctx);
   CK(io.copy_in(ctx->d_cost.p, vertex_costs, ctx->V));
@@ -855,6 +867,60 @@ static void fill_cvp_args(mnb_ctx* ctx, CvpKernelArgs& a) {
   a.hop = ctx->w_mean > 0 ? 1.35f * ctx->w_mean : 0.16f;
 }
 
+// A single plan's wave on the workspace of a.ws: k_cvp_grid or, with mnb_set_tuning(cluster >= 1), k_cvp<CS> -- in the
+// resumed form with RESUME (mnb_cvp_replan) -- then the epilogue.
+template <bool RESUME>
+static int32_t launch_single_cvp(mnb_ctx* ctx, CvpKernelArgs a) {
+  if (ctx->cluster == -1) {
+    a.delta = ctx->grid_delta;
+    if (ctx->grid_blocks_per_sm == 0) {
+      int nb = 0;
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_cvp_grid<false>, ctx->threads, 0));
+      ctx->grid_blocks_per_sm = nb > MNB_GRID_MINBLOCKS ? MNB_GRID_MINBLOCKS : nb;
+      if (nb <= 0) { ctx->err = "k_cvp_grid cannot be resident"; return MNB_E_CUDA; }
+    }
+    CK(launch_cooperative(k_cvp_grid<RESUME>, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
+  } else {
+    // k_cvp takes its query from the counter and bumps it again to leave its loop: every launch starts from zero
+    CK(cudaMemsetAsync(a.next_query, 0, sizeof(unsigned int), ctx->stream));
+    const cudaError_t e = with_cluster_size<16>(ctx->cluster, [&](auto c) {
+      constexpr int CS = decltype(c)::value;
+      return launch_cluster(k_cvp<CS, RESUME>, a, CS, (unsigned)CS, MNB_CVP_THREADS, ctx->stream);
+    });
+    if (e != cudaSuccess) { ctx->err = std::string("cvp launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
+  }
+  MNB_LAUNCH(k_cvp_epilogue, (ctx->V + 255) / 256, 256, 0, ctx->stream, a, a.ws.ctl);
+  CK(cudaGetLastError());
+  return MNB_OK;
+}
+
+// After the launches of a single plan: the copies back, the stats and the outcome (cvp:888-918); a plan that is not
+// cancelled becomes the last plan (mnb_cvp_backtrack, mnb_vector_map).
+static int32_t single_cvp_outcome(mnb_ctx* ctx, const CvpKernelArgs& a, CallerArrays& io, uint32_t seed_face, const float seed_pos[3],
+                                  int64_t robot_face, unsigned launches) {
+  int32_t rc;
+  CK(io.copy_back());
+  uint32_t rf[3] = {0, 0, 0}, rp[3] = {0, 0, 0};
+  if (robot_face >= 0) {
+    CK(cudaMemcpyAsync(rf, ctx->d_faces + 3 * (size_t)robot_face, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < 3; ++k)
+      CK(cudaMemcpyAsync(&rp[k], a.out_pred + rf[k], sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  ctx->last_valid = false;
+  if ((rc = finish_stats(ctx, 1, launches, a.ws.ctl)) != MNB_OK) return rc;
+  if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
+  ctx->last_pred = a.out_pred; ctx->last_dir = a.out_dir; ctx->last_cut = a.out_cut; ctx->last_seed_face = seed_face;
+  for (int k = 0; k < 3; ++k) ctx->last_seed_pos[k] = seed_pos[k];
+  ctx->last_valid = true;
+  if (robot_face >= 0) {
+    bool any = false;
+    for (int k = 0; k < 3; ++k) if (rp[k] != rf[k]) any = true;
+    if (!any && (uint32_t)robot_face != seed_face) return MNB_NO_PATH_FOUND;
+  }
+  return MNB_SUCCESS;
+}
+
 extern "C" {
 
 static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face, double cost_limit,
@@ -878,7 +944,6 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
   CK(cudaMemcpyAsync(ctx->d_seed_faces, &seed_face, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
   CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
   CvpKernelArgs a{};
   fill_cvp_args(ctx, a);
@@ -886,47 +951,102 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   a.sweeps = ctx->sweeps;
   a.out_dist = o_dist; a.out_pred = o_pred; a.out_dir = o_dir; a.out_cut = o_cut;
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  if (ctx->cluster == -1) {
-    a.delta = ctx->grid_delta;
-    if (ctx->grid_blocks_per_sm == 0) {
-      int nb = 0;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_cvp_grid, ctx->threads, 0));
-      ctx->grid_blocks_per_sm = nb > MNB_GRID_MINBLOCKS ? MNB_GRID_MINBLOCKS : nb;
-      if (nb <= 0) { ctx->err = "k_cvp_grid cannot be resident"; return MNB_E_CUDA; }
-    }
-    CK(launch_cooperative(k_cvp_grid, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
-  } else {
-    const cudaError_t e = with_cluster_size<16>(ctx->cluster, [&](auto c) {
-      constexpr int CS = decltype(c)::value;
-      return launch_cluster(k_cvp<CS>, a, CS, (unsigned)CS, MNB_CVP_THREADS, ctx->stream);
-    });
-    if (e != cudaSuccess) { ctx->err = std::string("cvp launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
-  }
-  MNB_LAUNCH(k_cvp_epilogue, (ctx->V + 255) / 256, 256, 0, ctx->stream, a, ctx->ws.ctl);
-  CK(cudaGetLastError());
+  if ((rc = launch_single_cvp<false>(ctx, a)) != MNB_OK) return rc;
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  CK(io.copy_back());
-  // outcome (cvp:888-918)
-  uint32_t rf[3] = {0, 0, 0}, rp[3] = {0, 0, 0};
-  if (robot_face >= 0) {
-    CK(cudaMemcpyAsync(rf, ctx->d_faces + 3 * (size_t)robot_face, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    for (int k = 0; k < 3; ++k)
-      CK(cudaMemcpyAsync(&rp[k], a.out_pred + rf[k], sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  ctx->last_valid = false;
-  if ((rc = finish_stats(ctx, 1, 2)) != MNB_OK) return rc;
-  if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
-  ctx->last_pred = a.out_pred; ctx->last_dir = a.out_dir; ctx->last_cut = a.out_cut; ctx->last_seed_face = seed_face;
-  for (int k = 0; k < 3; ++k) ctx->last_seed_pos[k] = seed_pos[k];
-  ctx->last_valid = true;
-  if (robot_face >= 0) {
-    bool any = false;
-    for (int k = 0; k < 3; ++k) if (rp[k] != rf[k]) any = true;
-    if (!any && (uint32_t)robot_face != seed_face) return MNB_NO_PATH_FOUND;
-  }
-  return MNB_SUCCESS;
+  return single_cvp_outcome(ctx, a, io, seed_face, seed_pos, robot_face, 2);
 }
+
+// mnb_cvp_replan: the arguments of mnb_cvp plus the union of the changed sets of the mnb_update_vertex_costs calls since
+// the resident wave.  The result is mnb_cvp's; the wave runs in the resident workspace and resumes from T0 when the last
+// successful replan had the same seed face, seed position and cost limit and only mnb_update_vertex_costs changed the
+// costs since (DESIGN §4, "Replan").  Otherwise, or when T0 is not after every seed's pop, or the level pool is more than
+// half full, or the resumed wave would overflow it, the call runs one whole wave there.
+static int32_t impl_cvp_replan(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face, double cost_limit,
+                               double goal_dist_offset, uint32_t n_changed, const uint32_t* changed,
+                               float* out_dist, uint32_t* out_pred, float* out_direction, int32_t* out_cut) {
+  if (!ctx || !seed_pos || !ctx->V || (n_changed && !changed)) return MNB_E_ARG;
+  const RepairRequest rq{n_changed, changed};
+  int32_t rc;
+  if ((rc = check_changed(ctx, &rq)) != MNB_OK) return rc;
+  if (!ctx->costs_set) { ctx->err = "mnb_set_costs / mnb_compute_edge_weights not called"; return MNB_E_STATE; }
+  if (seed_face >= ctx->F) return MNB_INVALID_START;
+  if (robot_face >= (int64_t)ctx->F) return MNB_INVALID_GOAL;
+  CK(cudaSetDevice(ctx->device));
+  const size_t V = ctx->V;
+  WaveBuffers& w = ctx->rw;
+  CK(w.state.reserve(V)); CK(w.ext.reserve(V)); CK(w.root.reserve(V)); CK(w.chg.reserve(V)); CK(w.ver.reserve(V));
+  CK(w.mark.reserve(V)); CK(w.list0.reserve(V)); CK(w.list1.reserve(V)); CK(w.pool.reserve(ws_pool_cap(ctx->V))); CK(w.ctl.reserve(1));
+  if ((rc = ensure_seeds(ctx, 1)) != MNB_OK) return rc;
+  CallerArrays io(ctx);
+  if ((rc = ensure_out(ctx, (io.device() && out_dist) ? 0 : V, true)) != MNB_OK) return rc;
+  float* const o_dist = io.needed(out_dist, ctx->d_out_dist.p, ctx->V);
+  uint32_t* const o_pred = io.needed(out_pred, ctx->d_out_pred.p, ctx->V);
+  float* const o_dir = io.needed(out_direction, ctx->d_out_dir.p, ctx->V);
+  int32_t* const o_cut = io.needed(out_cut, ctx->d_out_cut.p, ctx->V);
+  if (ctx->h_cancel) *ctx->h_cancel = 0;
+  CK(cudaMemcpyAsync(ctx->d_seed_faces, &seed_face, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->d_seed_pos, seed_pos, 3 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  CvpKernelArgs a{};
+  fill_cvp_args(ctx, a);
+  a.ws = WaveWorkspace{};
+  a.ws.state = w.state; a.ws.ext = w.ext; a.ws.root = w.root; a.ws.pool = w.pool; a.ws.pool_cap = ws_pool_cap(ctx->V);
+  a.ws.chg = w.chg; a.ws.ver = w.ver; a.ws.mark = w.mark; a.ws.list0 = w.list0; a.ws.list1 = w.list1; a.ws.ctl = w.ctl;
+  a.n_queries = 1; a.robot_face = robot_face; a.cost_limit = cost_limit; a.goal_dist_offset = goal_dist_offset;
+  a.sweeps = ctx->sweeps;
+  a.out_dist = o_dist; a.out_pred = o_pred; a.out_dir = o_dir; a.out_cut = o_cut;
+  uint32_t pos_bits[3]; uint64_t limit_bits;
+  std::memcpy(pos_bits, seed_pos, sizeof(pos_bits)); std::memcpy(&limit_bits, &cost_limit, sizeof(limit_bits));
+  bool resume = ctx->rw_valid && ctx->rw_seed_face == seed_face && std::equal(pos_bits, pos_bits + 3, ctx->rw_seed_pos) &&
+                ctx->rw_cost_limit == limit_bits && ctx->rw_cost_gen == ctx->cost_gen && ctx->rw_pool_top <= ws_pool_cap(ctx->V) / 2;
+  ctx->rw_valid = false;                       // until this call has succeeded
+  unsigned launches = 0;
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  if (resume) {
+    const unsigned blocks = std::max(1u, std::min((n_changed + 255u) / 256u, 2u * (unsigned)ctx->sm_count));
+    CK(ctx->d_replan_chg.reserve(std::max(1u, n_changed))); CK(ctx->d_replan_t0.reserve(REPLAN_T0_WORDS + 6 * (size_t)blocks));
+    if (n_changed) CK(cudaMemcpyAsync(ctx->d_replan_chg, changed, sizeof(uint32_t) * n_changed, cudaMemcpyHostToDevice, ctx->stream));
+    ReplanArgs r{};
+    r.V = ctx->V; r.faces = ctx->d_faces; r.cor_ptr = ctx->d_cor_ptr; r.cor_idx = ctx->d_cor_idx; r.cost = ctx->d_cost;
+    r.invalid = a.invalid; r.cost_limit = cost_limit; r.ws = a.ws; r.changed = ctx->d_replan_chg; r.n_changed = n_changed;
+    r.seed_face = seed_face; r.robot_face = robot_face; r.t0 = ctx->d_replan_t0;
+    MNB_LAUNCH(k_replan_t0, blocks, 256, 0, ctx->stream, r);
+    MNB_LAUNCH(k_replan_t0_final, 1, 256, 0, ctx->stream, r, blocks);
+    CK(cudaGetLastError());
+    launches += 2;
+    uint32_t ok = 0;
+    CK(cudaMemcpyAsync(&ok, ctx->d_replan_t0.p + 6, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    resume = ok != 0;
+    if (resume) {
+      const unsigned vb = (unsigned)((V + 255) / 256);
+      MNB_LAUNCH(k_replan_rollback, vb, 256, 0, ctx->stream, r);
+      MNB_LAUNCH(k_replan_frontier, vb, 256, 0, ctx->stream, r);
+      CK(cudaGetLastError());
+      CvpKernelArgs ra = a;
+      if (ctx->replan_pool_room) ra.ws.pool_cap = std::min<uint32_t>(ra.ws.pool_cap, ctx->rw_pool_top + ctx->replan_pool_room);
+      if ((rc = launch_single_cvp<true>(ctx, ra)) != MNB_OK) return rc;
+      launches += 4;
+      // the resumed wave allocates behind the old records: if the pool ran out, the whole wave starts from an empty one
+      unsigned int overflow = 0;
+      CK(cudaMemcpyAsync(&overflow, &a.ws.ctl->pool_overflow, sizeof(overflow), cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+      resume = overflow == 0;
+    }
+  }
+  if (!resume) {
+    CK(cudaMemsetAsync(a.ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
+    if ((rc = launch_single_cvp<false>(ctx, a)) != MNB_OK) return rc;
+    launches += 2;
+  }
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  rc = single_cvp_outcome(ctx, a, io, seed_face, seed_pos, robot_face, launches);
+  if (rc == MNB_SUCCESS || rc == MNB_NO_PATH_FOUND) {
+    ctx->rw_valid = true; ctx->rw_seed_face = seed_face; std::copy(pos_bits, pos_bits + 3, ctx->rw_seed_pos);
+    ctx->rw_cost_limit = limit_bits; ctx->rw_cost_gen = ctx->cost_gen; ctx->rw_pool_top = (uint32_t)ctx->stats.pool_words;
+  }
+  return rc;
+}
+
 
 // n full-field CVP plans in one launch, mnb_cvp_batch and mnb_cvp_batch_fields.  With vector-field outputs
 // (k_cvp_batch<CS, true>) each wavefront runs the epilogue of its goal before its group takes the next one; potentials
@@ -1267,6 +1387,10 @@ static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32
 
 // experiment knob (not part of the public header): in-round sweeps of the whole-grid single-plan kernel
 int32_t mnb_debug_set_sweeps(mnb_ctx* ctx, int32_t k) { if (!ctx || k < -1 || k > 64) return MNB_E_ARG; ctx->sweeps = k; return MNB_OK; }
+
+// test hook (not part of the public header): a resumed replan wave may add at most `words` level-pool words (0 = no limit
+// but the pool's), so that tests reach the whole-wave retry after a resumed wave ran out of pool
+int32_t mnb_debug_set_replan_pool_room(mnb_ctx* ctx, uint32_t words) { if (!ctx) return MNB_E_ARG; ctx->replan_pool_room = words; return MNB_OK; }
 
 int32_t mnb_debug_set_infl_skip(mnb_ctx* ctx, int32_t on) { if (!ctx) return MNB_E_ARG; ctx->infl_skip_clean = on != 0; return MNB_OK; }
 int32_t mnb_debug_set_layers_smem(mnb_ctx* ctx, int32_t mode) { if (!ctx || mode < 0 || mode > 9) return MNB_E_ARG; ctx->layers_smem = mode; ctx->layers_explicit = true; return MNB_OK; }
@@ -1655,6 +1779,12 @@ int32_t mnb_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* pos, con
 int32_t mnb_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face, double cost_limit,
                 double goal_dist_offset, float* out_dist, uint32_t* out_pred, float* out_direction, int32_t* out_cut) {
   return guarded(ctx, [&]() { return impl_cvp(ctx, seed_face, seed_pos, robot_face, cost_limit, goal_dist_offset, out_dist, out_pred, out_direction, out_cut); });
+}
+int32_t mnb_cvp_replan(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3], int64_t robot_face, double cost_limit,
+                       double goal_dist_offset, uint32_t n_changed, const uint32_t* changed, float* out_dist, uint32_t* out_pred,
+                       float* out_direction, int32_t* out_cut) {
+  return guarded(ctx, [&]() { return impl_cvp_replan(ctx, seed_face, seed_pos, robot_face, cost_limit, goal_dist_offset, n_changed, changed,
+                                                     out_dist, out_pred, out_direction, out_cut); });
 }
 int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
                              float* out_dist, uint32_t* out_pred, float* out_direction, int32_t* out_cutting_face) {
