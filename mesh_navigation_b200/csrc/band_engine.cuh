@@ -321,6 +321,18 @@ struct GroupCtl {               // one per wavefront group, global memory
   unsigned int done_ring[2];
 };
 
+// a pop time as six words, in the order of GroupCtl::goal_time: a1 bits, root, a2 bits, a3 bits, ext, vertex
+__device__ __forceinline__ void time_put(uint32_t* w, const EvTime& t) {
+  w[0] = __float_as_uint(t.a1); w[1] = t.root; w[2] = __float_as_uint(t.a2); w[3] = __float_as_uint(t.a3); w[4] = t.ext; w[5] = t.self;
+}
+__device__ __forceinline__ EvTime time_get(const uint32_t* w) {
+  EvTime t; t.a1 = __uint_as_float(__ldcg(&w[0])); t.root = __ldcg(&w[1]); t.a2 = __uint_as_float(__ldcg(&w[2]));
+  t.a3 = __uint_as_float(__ldcg(&w[3])); t.ext = __ldcg(&w[4]); t.self = __ldcg(&w[5]);
+  return t;
+}
+// later than every finite pop time
+__device__ __forceinline__ EvTime time_never() { return ev_normal(__uint_as_float(INF_BITS), 0xffffffffu); }
+
 // The matrix form of the batch kernels (mnb_dijkstra_matrix / mnb_cvp_matrix): a wave ends once every target vertex has
 // settled and writes only the labels of the targets.
 struct TargetSet {
@@ -392,6 +404,21 @@ __device__ __forceinline__ void stage_push_seen(Stage& st, SweepStage& ss, uint3
   stage_put_seen(st, ss, atomicAdd(&st.n, 1u), v, seen, label_bits, list_next, count_next);
 }
 
+// an empty stage (thread 0 of the CTA)
+template <class S>
+__device__ __forceinline__ void stage_init(S& st) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+
+// the warp minima of the threads' my_mtau / my_lo into the CTA stage (every lane of the warp calls this)
+template <class S>
+__device__ __forceinline__ void stage_reduce(S& st, float my_mtau, float my_lo) {
+  const unsigned int wm = __reduce_min_sync(0xffffffffu, __float_as_uint(my_mtau));
+  const unsigned int wl = __reduce_min_sync(0xffffffffu, __float_as_uint(my_lo));
+  if ((threadIdx.x & 31) == 0) {
+    if (wm != INF_BITS) atomicMin(&st.m_tau, wm);
+    if (wl != INF_BITS) atomicMin(&st.lo, wl);
+  }
+}
+
 // flush the CTA stage to the global list (all threads of the CTA call this)
 template <class S>
 __device__ __forceinline__ void stage_flush(S& st, uint32_t* list_next, unsigned int* count_next,
@@ -407,9 +434,44 @@ __device__ __forceinline__ void stage_flush(S& st, uint32_t* list_next, unsigned
   const unsigned int base = st.base;
   for (unsigned int i = threadIdx.x; i < n; i += blockDim.x) list_next[base + i] = st.buf[i];
   __syncthreads();
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  if (threadIdx.x == 0) stage_init(st);
   // no barrier needed here: the group barrier that follows every flush orders the reset
   // before the next round's pushes
+}
+
+// A vertex c with label `old` settles in round r: if it is the last of the robot face's vertices r0-r2 to settle, the goal
+// cutoff is armed at the latest pop time of the three (c is not necessarily the last of them in event order), and the
+// goal distance follows from that vertex's potential.
+template <class P>
+__device__ __forceinline__ void arm_goal_cutoff(const P& prob, GroupCtl* ctl, const int has_robot, const uint32_t r0, const uint32_t r1,
+                                                const uint32_t r2, const double goal_dist_offset, const uint32_t c, const Label& old, const uint32_t r) {
+  if (has_robot && (c == r0 || c == r1 || c == r2)) {
+    if (atomicSub(&ctl->robot_left, 1) == 1) {
+      float bd = old.d; EvTime bt = old.t;
+      const uint32_t rv[3] = {r0, r1, r2};
+      for (int k = 0; k < 3; ++k) {
+        const Label so = prob.load_label(rv[k]);
+        if (prob.tless(bt, so.t)) { bt = so.t; bd = so.d; }
+      }
+      time_put(ctl->goal_time, bt);
+      atomicMin(&ctl->goal_ring[(r + 1) & 1], __float_as_uint((float)((double)bd + goal_dist_offset)));
+    }
+  }
+}
+
+// the end of a wave after r rounds: the thread's counters, and (thread 0 of the group) the round count, the strict rule,
+// the watchdog and the final goal distance
+__device__ __forceinline__ void band_stats(GroupCtl* ctl, const uint32_t gtid, const uint32_t r, const uint32_t max_rounds, const int strict,
+                                           const unsigned long long recomputes, const unsigned long long settled, const unsigned long long skipped) {
+  atomicAdd(&ctl->recomputes, recomputes);
+  atomicAdd(&ctl->settled, settled);
+  if (skipped) atomicAdd(&ctl->skipped, skipped);
+  if (gtid == 0) {
+    ctl->rounds += r;
+    if (strict) ctl->strict_armed += 1;
+    if (r > max_rounds) ctl->watchdog = 1;
+    ctl->goal_bits = min(ctl->goal_ring[0], ctl->goal_ring[1]);
+  }
 }
 
 // -----------------------------------------------------------------------------
@@ -447,13 +509,9 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
     const float lo_prev = __uint_as_float(__ldcg(&ctl->lo[prev]));
     const unsigned int goal_b = __ldcg(&ctl->goal_ring[r & 1]);
     const float goal = __uint_as_float(goal_b);
-    if constexpr (P::HAS_GOAL_TIME) if (has_robot && goal_b != INF_BITS) {
-      prob.goal_t.a1 = __uint_as_float(__ldcg(&ctl->goal_time[0])); prob.goal_t.root = __ldcg(&ctl->goal_time[1]);
-      prob.goal_t.a2 = __uint_as_float(__ldcg(&ctl->goal_time[2])); prob.goal_t.a3 = __uint_as_float(__ldcg(&ctl->goal_time[3]));
-      prob.goal_t.ext = __ldcg(&ctl->goal_time[4]); prob.goal_t.self = __ldcg(&ctl->goal_time[5]);
-    }
+    if constexpr (P::HAS_GOAL_TIME) if (has_robot && goal_b != INF_BITS) prob.goal_t = time_get(ctl->goal_time);
     const unsigned int stop = __ldcg(&ctl->stop_ring[r & 1]);
-    if (n == 0 || stop || r > max_rounds) break;   // r is group-uniform: the watchdog cannot deadlock the barrier
+    if (n == 0 || stop || r > max_rounds) break;  // r is group-uniform: the watchdog cannot deadlock the barrier
     // every target has settled.  The flag needs no carrying or clearing: the loop ends at the first round that reads it
     // raised, so slot (r+1)&1 was read clear in round r-1 and nobody has written it since.
     if constexpr (TARGETS) if (__ldcg(&ctl->done_ring[r & 1])) break;
@@ -561,7 +619,7 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
     for (unsigned int i = gtid; i < n; i += gthreads) {
       const uint32_t c = __ldcg(&list_r[i]);
       const Label old = prob.load_label(c);
-      const float d = old.d, tau = old.t.a1;
+      const float tau = old.t.a1;
       // a vertex that is never fixed (inflation: invalid vertices pop without being fixed, inflation_layer.cpp:417-422) keeps
       // receiving updates from faces that fire AFTER its own pop: its label is not a function of earlier events only, so it
       // stays a candidate until a whole round went by without any change, and it does not hold the band back
@@ -571,48 +629,19 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
         mark[c] = MARK_FIXED;
         my_settled++;
         if constexpr (TARGETS) settle_target(ctl, target_bits, c, r);
-        if (has_robot && (c == r0 || c == r1 || c == r2)) {
-          if (atomicSub(&ctl->robot_left, 1) == 1) {
-            // c is not necessarily the last of the three in event order: take the latest pop time
-            float bd = d; EvTime bt = old.t;
-            const uint32_t rv[3] = {r0, r1, r2};
-            for (int k = 0; k < 3; ++k) {
-              const Label so = prob.load_label(rv[k]);
-              if (prob.tless(bt, so.t)) { bt = so.t; bd = so.d; }
-            }
-            ctl->goal_time[0] = __float_as_uint(bt.a1); ctl->goal_time[1] = bt.root; ctl->goal_time[2] = __float_as_uint(bt.a2);
-            ctl->goal_time[3] = __float_as_uint(bt.a3); ctl->goal_time[4] = bt.ext; ctl->goal_time[5] = bt.self;
-            atomicMin(&ctl->goal_ring[(r + 1) & 1], __float_as_uint((float)((double)bd + goal_dist_offset)));
-          }
-        }
+        arm_goal_cutoff(prob, ctl, has_robot, r0, r1, r2, goal_dist_offset, c, old, r);
         continue;
       }
       evaluate(c, old, nf);
     }
-    {
-      my_mtau = fminf(my_mtau, prob.deferred_m);      // deferred back-steps are pending changes
-      prob.deferred_m = __uint_as_float(INF_BITS);
-      const unsigned int wm = __reduce_min_sync(0xffffffffu, __float_as_uint(my_mtau));
-      const unsigned int wl = __reduce_min_sync(0xffffffffu, __float_as_uint(my_lo));
-      if ((threadIdx.x & 31) == 0) {
-        if (wm != INF_BITS) atomicMin(&st.m_tau, wm);
-        if (wl != INF_BITS) atomicMin(&st.lo, wl);
-      }
-    }
+    my_mtau = fminf(my_mtau, prob.deferred_m);      // deferred back-steps are pending changes
+    prob.deferred_m = __uint_as_float(INF_BITS);
+    stage_reduce(st, my_mtau, my_lo);
     stage_flush(st, list_n, &ctl->count[next], &ctl->m_tau[slot], &ctl->lo[slot]);
     band_end_prev = band_end;
     group_sync<CS>(ctl->barrier);
   }
-  // statistics
-  atomicAdd(&ctl->recomputes, my_recomputes);
-  atomicAdd(&ctl->settled, my_settled);
-  if (my_skipped) atomicAdd(&ctl->skipped, my_skipped);
-  if (gtid == 0) {
-    ctl->rounds += r;
-    if (prob.strict) ctl->strict_armed += 1;
-    if (r > max_rounds) ctl->watchdog = 1;
-    ctl->goal_bits = min(ctl->goal_ring[0], ctl->goal_ring[1]);
-  }
+  band_stats(ctl, gtid, r, max_rounds, prob.strict, my_recomputes, my_settled, my_skipped);
 }
 
 // -----------------------------------------------------------------------------
@@ -652,11 +681,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     const float lo_prev = __uint_as_float(__ldcg(&ctl->lo[prev]));
     const unsigned int goal_b = __ldcg(&ctl->goal_ring[r & 1]);
     const float goal = __uint_as_float(goal_b);
-    if constexpr (P::HAS_GOAL_TIME) if (has_robot && goal_b != INF_BITS) {
-      prob.goal_t.a1 = __uint_as_float(__ldcg(&ctl->goal_time[0])); prob.goal_t.root = __ldcg(&ctl->goal_time[1]);
-      prob.goal_t.a2 = __uint_as_float(__ldcg(&ctl->goal_time[2])); prob.goal_t.a3 = __uint_as_float(__ldcg(&ctl->goal_time[3]));
-      prob.goal_t.ext = __ldcg(&ctl->goal_time[4]); prob.goal_t.self = __ldcg(&ctl->goal_time[5]);
-    }
+    if constexpr (P::HAS_GOAL_TIME) if (has_robot && goal_b != INF_BITS) prob.goal_t = time_get(ctl->goal_time);
     const unsigned int stop = __ldcg(&ctl->stop_ring[r & 1]);
     // the round in which the goal cutoff first becomes visible must run even if nothing else is left to do: it puts the
     // vertices that settled beyond the cutoff back into the list (see below)
@@ -783,19 +808,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     auto settle = [&](const uint32_t c, const Label& old) {
       mark[c] = MARK_FIXED;
       my_settled++;
-      if (has_robot && (c == r0 || c == r1 || c == r2)) {
-        if (atomicSub(&ctl->robot_left, 1) == 1) {
-          float bd = old.d; EvTime bt = old.t;
-          const uint32_t rv[3] = {r0, r1, r2};
-          for (int k = 0; k < 3; ++k) {
-            const Label so = prob.load_label(rv[k]);
-            if (prob.tless(bt, so.t)) { bt = so.t; bd = so.d; }
-          }
-          ctl->goal_time[0] = __float_as_uint(bt.a1); ctl->goal_time[1] = bt.root; ctl->goal_time[2] = __float_as_uint(bt.a2);
-          ctl->goal_time[3] = __float_as_uint(bt.a3); ctl->goal_time[4] = bt.ext; ctl->goal_time[5] = bt.self;
-          atomicMin(&ctl->goal_ring[(r + 1) & 1], __float_as_uint((float)((double)bd + goal_dist_offset)));
-        }
-      }
+      arm_goal_cutoff(prob, ctl, has_robot, r0, r1, r2, goal_dist_offset, c, old, r);
     };
     const unsigned int cnt = n > blk ? (n - blk + nblk - 1) / nblk : 0u;
     // the 8-lane main pass over cnt_g candidates: the CTA's share of the round's list or (queued) the entries of gq
@@ -975,16 +988,9 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       if (gtid == 0) ctl->t_ph[6] += (unsigned long long)(clock64() - tq1);
 #endif
     }
-    {
-      my_mtau = fminf(my_mtau, prob.deferred_m);      // deferred back-steps are pending changes
-      prob.deferred_m = __uint_as_float(INF_BITS);
-      const unsigned int wm = __reduce_min_sync(0xffffffffu, __float_as_uint(my_mtau));
-      const unsigned int wl = __reduce_min_sync(0xffffffffu, __float_as_uint(my_lo));
-      if ((threadIdx.x & 31) == 0) {
-        if (wm != INF_BITS) atomicMin(&st.m_tau, wm);
-        if (wl != INF_BITS) atomicMin(&st.lo, wl);
-      }
-    }
+    my_mtau = fminf(my_mtau, prob.deferred_m);      // deferred back-steps are pending changes
+    prob.deferred_m = __uint_as_float(INF_BITS);
+    stage_reduce(st, my_mtau, my_lo);
     __syncthreads();
 #ifdef MNB_GRID_TIMING
     const long long tp1 = clock64();
@@ -999,14 +1005,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     if (gtid == 0) { const long long tp3 = clock64(); ctl->t_work += (unsigned long long)(tp1 - tp0); ctl->t_flush += (unsigned long long)(tp2 - tp1); ctl->t_sync += (unsigned long long)(tp3 - tp2); }
 #endif
   }
-  atomicAdd(&ctl->recomputes, my_recomputes);
-  atomicAdd(&ctl->settled, my_settled);
-  if (gtid == 0) {
-    ctl->rounds += r;
-    if (prob.strict) ctl->strict_armed += 1;
-    if (r > max_rounds) ctl->watchdog = 1;
-    ctl->goal_bits = min(ctl->goal_ring[0], ctl->goal_ring[1]);
-  }
+  band_stats(ctl, gtid, r, max_rounds, prob.strict, my_recomputes, my_settled, 0ull);
 }
 
 }  // namespace mnb

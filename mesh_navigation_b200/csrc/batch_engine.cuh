@@ -18,7 +18,6 @@
 
 namespace mnb {
 
-struct BatchSeeds { uint32_t s0, s1, s2, noexpand; float seed_max; };
 constexpr uint32_t LIST_ACTIVATED = 0x80000000u;
 
 struct BatchGroup {          // per-wavefront pointers (group g of the workspace)
@@ -27,22 +26,15 @@ struct BatchGroup {          // per-wavefront pointers (group g of the workspace
 };
 
 template <class Args>
-__device__ __forceinline__ void batch_make_problem(const Args& a, const BatchGroup& G, const BatchSeeds& sd, int strict,
+__device__ __forceinline__ void batch_make_problem(const Args& a, const BatchGroup& G, const SeedFace& sd, int strict,
                                                    CvpEllProblem& prob) {
-  prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
-  prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo;
-  prob.state = G.state; prob.ext_arr = G.ext_arr; prob.root_arr = G.root_arr; prob.chg = G.chg;
-  prob.pool_w = G.pool; prob.pool = G.pool; prob.pool_cap = G.pool_cap; prob.pool_top = &G.ctl->pool_top; prob.pool_overflow = &G.ctl->pool_overflow;
-  prob.ver = nullptr; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = nullptr; prob.dir = nullptr; prob.cut = nullptr;
-  prob.cost_limit = a.cost_limit; prob.s0 = sd.s0; prob.s1 = sd.s1; prob.s2 = sd.s2; prob.seed_noexpand = sd.noexpand; prob.seed_max_d = sd.seed_max;
-  prob.goal_t = ev_normal(__uint_as_float(INF_BITS), 0u);
-  prob.prefetch_marks = false;
+  cvp_ell_problem(a, G.state, G.ext_arr, G.root_arr, G.chg, G.pool, G.pool_cap, G.ctl, sd, ev_normal(__uint_as_float(INF_BITS), 0u), false, prob);
   prob.strict = strict;
 }
 
 // the generic 8-lane evaluation (every lane of the warp calls this; groups that do not need it pass has = false)
 template <class Args>
-__device__ __noinline__ void batch_slow_eval(const Args& a, const BatchGroup& G, const BatchSeeds& sd, int strict, uint32_t c, uint32_t j,
+__device__ __noinline__ void batch_slow_eval(const Args& a, const BatchGroup& G, const SeedFace& sd, int strict, uint32_t c, uint32_t j,
                                              bool has, const int4& ix, const float4& w, float band_end, uint32_t round, const uint4& old_bits,
                                              float& nd, EvTime& nt, float& deferred_m) {
   CvpEllProblem prob;
@@ -55,7 +47,7 @@ __device__ __noinline__ void batch_slow_eval(const Args& a, const BatchGroup& G,
 
 // store of a label that is not plain (cascade member): compares with the old label, returns "changed"
 template <class Args>
-__device__ __noinline__ bool batch_store_general(const Args& a, const BatchGroup& G, const BatchSeeds& sd, uint32_t c, uint32_t j, bool has,
+__device__ __noinline__ bool batch_store_general(const Args& a, const BatchGroup& G, const SeedFace& sd, uint32_t c, uint32_t j, bool has,
                                                  const uint4& old_bits, float nd, const EvTime& nt, uint32_t round) {
   if (!has) return false;
   CvpEllProblem prob;
@@ -108,7 +100,7 @@ struct BatchWork { static constexpr int CAP = 2048; uint32_t q[CAP]; uint32_t sq
 // the sources, possible seeds, non-causal faces that may fire first, more than 8 faces, strict rounds.  A few percent of
 // the evaluations; kept out of line so that its register needs do not weigh on the throughput phases.
 template <class Args>
-__device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup& G, const BatchSeeds& sd, BatchStage& st, BatchWork& wk,
+__device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup& G, const SeedFace& sd, BatchStage& st, BatchWork& wk,
                                                  uint32_t* list_n, unsigned int* count_next, const float band_end, const int strict, const uint32_t r,
                                                  float& my_mtau_io, float& my_lo_io, unsigned int& my_recomputes_io) {
   constexpr unsigned FULL = 0xffffffffu;
@@ -269,7 +261,7 @@ __device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup
 template <int CS, bool TARGETS = false, class Args>
 __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const BatchGroup& G, uint32_t* list0, uint32_t* list1, BatchStage& st,
                                                       BatchWork& wk, const float delta, const uint32_t gthreads, const uint32_t gtid,
-                                                      const BatchSeeds& sd, const float band_end_init) {
+                                                      const SeedFace& sd, const float band_end_init) {
   constexpr unsigned FULL = 0xffffffffu;
   const float INF = __uint_as_float(INF_BITS);
   GroupCtl* const ctl = G.ctl;
@@ -444,14 +436,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
       if (threadIdx.x == 0) { wk.n = 0; wk.ns = 0; }
       __syncthreads();
     }     // chunks
-    {
-      const unsigned int wm = __reduce_min_sync(FULL, __float_as_uint(my_mtau));
-      const unsigned int wl = __reduce_min_sync(FULL, __float_as_uint(my_lo));
-      if (lane == 0) {
-        if (wm != INF_BITS) atomicMin(&st.m_tau, wm);
-        if (wl != INF_BITS) atomicMin(&st.lo, wl);
-      }
-    }
+    stage_reduce(st, my_mtau, my_lo);
     {   // statistics: one atomic per warp and round
       const unsigned int wr = __reduce_add_sync(FULL, my_recomputes), ws = __reduce_add_sync(FULL, my_settled), wk2 = __reduce_add_sync(FULL, my_skipped);
       if (lane == 0) {

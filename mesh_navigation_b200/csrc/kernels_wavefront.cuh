@@ -75,9 +75,47 @@ __device__ __forceinline__ void ctl_reset(GroupCtl* ctl, unsigned int n0, float 
   ctl->lo[0] = INF_BITS; ctl->lo[1] = INF_BITS; ctl->lo[2] = __float_as_uint(seed_min);
   ctl->goal_ring[0] = INF_BITS; ctl->goal_ring[1] = INF_BITS; ctl->stop_ring[0] = 0; ctl->stop_ring[1] = 0;
   ctl->goal_bits = INF_BITS; ctl->robot_left = 0;
-  ctl->goal_time[0] = INF_BITS; ctl->goal_time[1] = 0u; ctl->goal_time[2] = 0u; ctl->goal_time[3] = 0u; ctl->goal_time[4] = 0u; ctl->goal_time[5] = 0u;
+  time_put(ctl->goal_time, ev_normal(__uint_as_float(INF_BITS), 0u));
   ctl->pool_top = 0u;
   ctl->done_ring[0] = 0u; ctl->done_ring[1] = 0u;
+}
+
+// the label of a seed with potential d (its pop time is (d, seed)): the engine's 16-byte word or the lean float label
+__device__ __forceinline__ void put_seed_label(uint4& w, float d) { w = make_uint4(__float_as_uint(d), __float_as_uint(d), 0u, 0u); }
+__device__ __forceinline__ void put_seed_label(float& w, float d) { w = d; }
+
+// The seeding of a fresh wave (one thread): the n seeds s[k] take their labels d[k] and are fixed, their eligible
+// neighbours are the first candidates in list 0, and the control block is reset with the band at lo_init.
+template <class P>
+__device__ __forceinline__ void seed_wave(const P& prob, GroupCtl* ctl, uint32_t* mark, uint32_t* list0, const uint32_t* s, const float* d,
+                                          int n, float lo_init) {
+  for (int k = 0; k < n; ++k) { put_seed_label(prob.state[s[k]], d[k]); mark[s[k]] = MARK_FIXED; }
+  unsigned int n0 = 0;
+  for (int k = 0; k < n; ++k)
+    prob.activate(s[k], [&](uint32_t x) {
+      if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
+    });
+  ctl_reset(ctl, n0, lo_init);
+}
+
+// The fields every CvpProblem sets: the mesh tables, costs, gates and cost limit of a; the label store of one workspace
+// group (its labels, side arrays, level pool and control block); the seed face; the goal cutoff's pop time (+inf: not
+// armed); the outputs (any may be null).  No in-round sweeps (ver), strict rule off.
+__device__ __forceinline__ void cvp_problem(const CvpKernelArgs& a, uint4* state, uint32_t* ext, uint32_t* root, uint32_t* chg, uint32_t* pool,
+                                            uint32_t pool_cap, GroupCtl* ctl, const SeedFace& sd, const EvTime& goal_t, uint32_t* pred, float* dir, int32_t* cut,
+                                            CvpProblem& prob) {
+  prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid; prob.cost_limit = a.cost_limit;
+  prob.state = state; prob.ext_arr = ext; prob.root_arr = root; prob.chg = chg;
+  prob.pool_w = pool; prob.pool = pool; prob.pool_cap = pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
+  prob.s0 = sd.s[0]; prob.s1 = sd.s[1]; prob.s2 = sd.s[2]; prob.seed_noexpand = sd.noexpand; prob.seed_max_d = sd.seed_max;
+  prob.goal_t = goal_t; prob.pred = pred; prob.dir = dir; prob.cut = cut;
+  prob.ver = nullptr; prob.deferred_m = __uint_as_float(INF_BITS); prob.strict = 0;
+}
+// ... and the ELL tables of the 8-lane form (no outputs: the wavefront writes labels only)
+__device__ __forceinline__ void cvp_ell_problem(const CvpKernelArgs& a, uint4* state, uint32_t* ext, uint32_t* root, uint32_t* chg, uint32_t* pool,
+                                                uint32_t pool_cap, GroupCtl* ctl, const SeedFace& sd, const EvTime& goal_t, bool prefetch_marks, CvpEllProblem& prob) {
+  cvp_problem(a, state, ext, root, chg, pool, pool_cap, ctl, sd, goal_t, nullptr, nullptr, nullptr, prob);
+  prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo; prob.prefetch_marks = prefetch_marks;
 }
 
 // Matrix form, after the seeding (and a group barrier): ctl->targets_left = tg.distinct less the targets that are done
@@ -108,108 +146,68 @@ __device__ __forceinline__ void count_targets_done_at_init(const TargetSet& tg, 
 #ifndef MNB_CVP_THREADS
 #define MNB_CVP_THREADS 512
 #endif
-// RESUME (mnb_cvp_replan, single plan): the workspace holds a rolled-back wave (k_replan_rollback, k_replan_frontier), so
-// the clearing pass and the seeding are skipped and the band starts at T0 (DESIGN §4, "Replan").
+// The prologue of a single-plan CVP wave (k_cvp, k_cvp_grid): the clearing pass (the sweep versions only for the kernel
+// with in-round sweeps), the problem, and -- unless RESUME -- the seeding; then the robot face's vertices rv (none:
+// 0xffffffff) and how many of them are not fixed.  If none is left, the robot face is the seed face and the cutoff is armed
+// when the last seed pops (cvp:763-771).  Called by every thread of the group; ends with a group barrier.
+template <int CS, bool RESUME>
+__device__ __forceinline__ void cvp_single_setup(const CvpKernelArgs& a, bool clear_ver, bool prefetch_marks, uint32_t gthreads, uint32_t gtid,
+                                                 CvpEllProblem& prob, uint32_t (&rv)[3]) {
+  uint4* state = a.ws.state; uint32_t* mark = a.ws.mark; GroupCtl* ctl = a.ws.ctl;
+  if constexpr (!RESUME) {
+    for (uint32_t v = gtid; v < a.V; v += gthreads) {
+      state[v] = state_inf(); mark[v] = MARK_NONE; a.ws.chg[v] = 0u;
+      if (clear_ver) a.ws.ver[v] = 0u;
+    }
+    group_sync<CS>();
+  }
+  const CvpSeeds sd = cvp_seeds(a.faces, a.pos, a.cost, a.invalid, a.cost_limit, a.seed_faces[0], a.seed_pos);
+  cvp_ell_problem(a, state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, a.ws.pool_cap, ctl, sd, ev_normal(__uint_as_float(INF_BITS), 0u), prefetch_marks, prob);
+  prob.ver = a.ws.ver;
+  const bool has_robot = a.robot_face >= 0;
+  for (int k = 0; k < 3; ++k) rv[k] = has_robot ? a.faces[3 * (size_t)a.robot_face + k] : 0xffffffffu;
+  if (gtid == 0) {
+    if constexpr (!RESUME) seed_wave(prob, ctl, mark, a.ws.list0, sd.s, sd.d, 3, sd.seed_min);
+    if (has_robot) {
+      int left = 0;
+      for (int k = 0; k < 3; ++k) if (mark[rv[k]] != MARK_FIXED) left++;
+      ctl->robot_left = left;
+      if (left == 0) {
+        ctl->goal_ring[0] = __float_as_uint((float)((double)sd.seed_max + a.goal_dist_offset));
+        uint32_t sl = sd.s[0]; float sdl = sd.d[0];
+        for (int k = 1; k < 3; ++k) if (sd.d[k] > sdl || (sd.d[k] == sdl && sd.s[k] > sl)) { sl = sd.s[k]; sdl = sd.d[k]; }
+        time_put(ctl->goal_time, ev_normal(sdl, sl));
+      }
+    }
+  }
+  group_sync<CS>();
+}
+
+// A single plan on one cluster of CS CTAs (mnb_set_tuning(cluster >= 1)).
+// RESUME (mnb_cvp_replan): the workspace holds a rolled-back wave (k_replan_rollback, k_replan_frontier), so the clearing
+// pass and the seeding are skipped and the band starts at T0 (DESIGN §4, "Replan").
 template <int CS, bool RESUME = false>
 __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(const CvpKernelArgs a) {
   __shared__ Stage st;
   uint32_t g, gthreads, gtid;
   group_coords<CS>(g, gthreads, gtid);
-  const uint32_t V = a.V;
-  uint4* state = a.ws.state + (size_t)g * V;
-  uint32_t* mark = a.ws.mark + (size_t)g * V;
-  uint32_t* list0 = a.ws.list0 + (size_t)g * V;
-  uint32_t* list1 = a.ws.list1 + (size_t)g * V;
-  GroupCtl* ctl = a.ws.ctl + g;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  GroupCtl* ctl = a.ws.ctl;
+  if (threadIdx.x == 0) stage_init(st);
   __syncthreads();
-
-  for (;;) {
-    if (gtid == 0) ctl->query = atomicAdd(a.next_query, 1u);
-    group_sync<CS>();
-    const uint32_t q = __ldcg(&ctl->query);
-    if (q >= a.n_queries) break;
-    const bool single = (a.n_queries == 1);
-    uint32_t* chg = a.ws.chg + (size_t)g * V;
-    const int sweeps = 0;                            // in-round sweeps are compiled into the whole-grid kernel only
-    if constexpr (!RESUME) {
-      for (uint32_t v = gtid; v < V; v += gthreads) {
-        state[v] = state_inf(); mark[v] = MARK_NONE; chg[v] = 0u;
-        if (sweeps) a.ws.ver[v] = 0u;
-      }
-      group_sync<CS>();
-    }
-
-    const uint32_t sf = a.seed_faces[q];
-    const uint32_t s0 = a.faces[3 * (size_t)sf], s1 = a.faces[3 * (size_t)sf + 1], s2 = a.faces[3 * (size_t)sf + 2];
-    CvpEllProblem prob;
-    prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
-    prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo;
-    prob.state = state; prob.ext_arr = a.ws.ext + (size_t)g * V; prob.root_arr = a.ws.root + (size_t)g * V; prob.chg = chg;
-    prob.pool_w = a.ws.pool + (size_t)g * a.ws.pool_cap; prob.pool = prob.pool_w; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
-    prob.ver = a.ws.ver; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = nullptr; prob.dir = nullptr; prob.cut = nullptr; prob.cost_limit = a.cost_limit;
-    prob.s0 = s0; prob.s1 = s1; prob.s2 = s2; prob.seed_noexpand = 0; prob.goal_t = ev_normal(__uint_as_float(INF_BITS), 0u);
-    prob.prefetch_marks = false;
-    float sd[3];
-    {
-      const uint32_t sv[3] = {s0, s1, s2};
-      for (int k = 0; k < 3; ++k) {   // cvp:719-728
-        const float dx = a.seed_pos[3 * (size_t)q] - a.pos[3 * (size_t)sv[k]];
-        const float dy = a.seed_pos[3 * (size_t)q + 1] - a.pos[3 * (size_t)sv[k] + 1];
-        const float dz = a.seed_pos[3 * (size_t)q + 2] - a.pos[3 * (size_t)sv[k] + 2];
-        sd[k] = sqrtf(dx * dx + dy * dy + dz * dz);
-        const bool noexp = ((double)a.cost[sv[k]] >= a.cost_limit) || (a.invalid && a.invalid[sv[k]]);  // cvp:757,760
-        if (noexp) prob.seed_noexpand |= (1u << k);
-      }
-    }
-    const float seed_min = fminf(sd[0], fminf(sd[1], sd[2]));
-    const float seed_max = fmaxf(sd[0], fmaxf(sd[1], sd[2]));
-    prob.seed_max_d = seed_max;
-    uint32_t r0 = 0xffffffffu, r1 = 0xffffffffu, r2 = 0xffffffffu;
-    const int has_robot = single && a.robot_face >= 0;
-    if (has_robot) {
-      r0 = a.faces[3 * (size_t)a.robot_face]; r1 = a.faces[3 * (size_t)a.robot_face + 1]; r2 = a.faces[3 * (size_t)a.robot_face + 2];
-    }
-    if (gtid == 0) {
-      const uint32_t sv[3] = {s0, s1, s2};
-      if constexpr (!RESUME) {
-        for (int k = 0; k < 3; ++k) {
-          state[sv[k]] = make_uint4(__float_as_uint(sd[k]), __float_as_uint(sd[k]), 0u, 0u);
-          mark[sv[k]] = MARK_FIXED;
-        }
-        unsigned int n0 = 0;
-        for (int k = 0; k < 3; ++k)
-          prob.activate(sv[k], [&](uint32_t x) {
-            if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-          });
-        ctl_reset(ctl, n0, seed_min);
-      }
-      if (has_robot) {
-        int left = 0; const uint32_t rv[3] = {r0, r1, r2};
-        for (int k = 0; k < 3; ++k) if (mark[rv[k]] != MARK_FIXED) left++;
-        ctl->robot_left = left;
-        if (left == 0) {  // robot face == seed face: cutoff armed when the last seed pops (cvp:763-771)
-          ctl->goal_ring[0] = __float_as_uint((float)((double)seed_max + a.goal_dist_offset));
-          uint32_t sl = sv[0]; float sdl = sd[0];
-          for (int k = 1; k < 3; ++k) if (sd[k] > sdl || (sd[k] == sdl && sv[k] > sl)) { sl = sv[k]; sdl = sd[k]; }
-          ctl->goal_time[0] = __float_as_uint(sdl); ctl->goal_time[1] = sl; ctl->goal_time[5] = sl;
-        }
-      }
-    }
-    group_sync<CS>();
-    float delta = a.delta;
-    if (has_robot && a.goal_dist_offset < (double)delta) delta = (float)fmax(a.goal_dist_offset, 1e-4);
-    // a resumed band starts at T0: every kept label (and seed) lies below it (k_replan_rollback set lo[2] = T0's key)
-    const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : seed_max;
-    run_band_rounds_sub8<CS, false, CvpEllProblem, RESUME>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, r0, r1, r2,
-                        a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)), a.max_rounds, sweeps, nullptr, V);
-    group_sync<CS>();
-    if (a.out_dist) {
-      float* od = a.out_dist + (size_t)q * V;
-      for (uint32_t v = gtid; v < V; v += gthreads) od[v] = __uint_as_float(state[v].x);
-    }
-    group_sync<CS>();
-  }
+  CvpEllProblem prob;
+  uint32_t rv[3];
+  cvp_single_setup<CS, RESUME>(a, false, false, gthreads, gtid, prob, rv);
+  const int has_robot = a.robot_face >= 0;
+  float delta = a.delta;
+  if (has_robot && a.goal_dist_offset < (double)delta) delta = (float)fmax(a.goal_dist_offset, 1e-4);
+  // a resumed band starts at T0: every kept label (and seed) lies below it (k_replan_rollback set lo[2] = T0's key)
+  const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : prob.seed_max_d;
+  run_band_rounds_sub8<CS, false, CvpEllProblem, RESUME>(prob, ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, has_robot,
+                        rv[0], rv[1], rv[2], a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)),
+                        a.max_rounds, 0, nullptr, a.V);     // in-round sweeps are compiled into the whole-grid kernel only
+  group_sync<CS>();
+  if (a.out_dist)
+    for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
 }
 
 // Batches of full-field plans (mnb_cvp_batch): the lean round loop of batch_engine.cuh.  One wavefront per CTA (CS = 1) or
@@ -225,22 +223,14 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
 // Every vertex replays its faces once more in event order and evaluates the winning face with the literal acos form.  Done
 // after the wavefront so that the stored angles use the final source potentials.  Run by k_cvp_epilogue for a single plan
 // and by k_cvp_batch<CS, true> for each goal of a batch, on the wavefront's own workspace group.
-// The problem object: the workspace group's labels, the goal's seed face sf, the goal cutoff's pop time (not armed: +inf)
-// and the outputs (any may be null).
+// The problem object: the workspace group's labels, the goal's seed face sf (seed point sp), the goal cutoff's pop time (not
+// armed: +inf) and the outputs (any may be null).
 __device__ __forceinline__ void cvp_epilogue_problem(const CvpKernelArgs& a, uint4* state, uint32_t* ext, uint32_t* root, uint32_t* chg,
-                                                     uint32_t* pool, GroupCtl* ctl, uint32_t sf, const EvTime& goal_t,
+                                                     uint32_t* pool, GroupCtl* ctl, uint32_t sf, const float* sp, const EvTime& goal_t,
                                                      uint32_t* pred, float* dir, int32_t* cut, CvpProblem& prob) {
-  prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
-  prob.state = state; prob.ext_arr = ext; prob.root_arr = root; prob.chg = chg;
-  prob.pool_w = pool; prob.pool = pool; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
-  prob.ver = nullptr; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = pred; prob.dir = dir; prob.cut = cut; prob.cost_limit = a.cost_limit;
-  prob.strict = 0;
-  prob.s0 = a.faces[3 * (size_t)sf]; prob.s1 = a.faces[3 * (size_t)sf + 1]; prob.s2 = a.faces[3 * (size_t)sf + 2];
-  prob.seed_noexpand = 0;
-  prob.goal_t = goal_t;
-  const uint32_t sv[3] = {prob.s0, prob.s1, prob.s2};
-  for (int k = 0; k < 3; ++k)
-    if (((double)a.cost[sv[k]] >= a.cost_limit) || (a.invalid && a.invalid[sv[k]])) prob.seed_noexpand |= (1u << k);
+  SeedFace sd = cvp_seeds(a.faces, a.pos, a.cost, a.invalid, a.cost_limit, sf, sp);
+  sd.seed_max = __builtin_huge_valf();       // final labels: the replay tests every source for a seed
+  cvp_problem(a, state, ext, root, chg, pool, a.ws.pool_cap, ctl, sd, goal_t, pred, dir, cut, prob);
 }
 
 // one vertex c of the epilogue (goal: the goal cutoff's potential, +inf when not armed)
@@ -268,7 +258,7 @@ __device__ __noinline__ void batch_fields_epilogue(const CvpKernelArgs& a, const
   const size_t row = (size_t)q * V;
   const uint32_t sf = a.seed_faces[q];
   CvpProblem prob;
-  cvp_epilogue_problem(a, G.state, G.ext_arr, G.root_arr, G.chg, G.pool, G.ctl, sf, ev_normal(__uint_as_float(INF_BITS), 0u),
+  cvp_epilogue_problem(a, G.state, G.ext_arr, G.root_arr, G.chg, G.pool, G.ctl, sf, a.seed_pos + 3 * (size_t)q, ev_normal(__uint_as_float(INF_BITS), 0u),
                        a.out_pred ? a.out_pred + row : nullptr, a.out_dir ? a.out_dir + row : nullptr, a.out_cut ? a.out_cut + row : nullptr, prob);
   for (uint32_t v = gtid; v < V; v += gthreads) cvp_epilogue_vertex(prob, G.ctl, sf, __uint_as_float(INF_BITS), v);
 }
@@ -294,7 +284,7 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
   uint32_t* list0 = a.ws.list0 + (size_t)g * V;
   uint32_t* list1 = a.ws.list1 + (size_t)g * V;
   GroupCtl* ctl = G.ctl;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; wk.n = 0; wk.ns = 0; }
+  if (threadIdx.x == 0) { stage_init(st); wk.n = 0; wk.ns = 0; }
   __syncthreads();
   for (;;) {
     if (gtid == 0) {
@@ -306,48 +296,30 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
     if (q >= a.n_queries) break;
     for (uint32_t v = gtid; v < V; v += gthreads) { G.state[v] = state_inf(); G.mark[v] = MARK_NONE; G.chg[v] = 0u; G.skipw[v] = make_uint4(INF_BITS, INF_BITS, 0u, 0u); }
     group_sync<CS>();
-    const uint32_t sf = a.seed_faces[q];
-    BatchSeeds sd;
-    sd.s0 = a.faces[3 * (size_t)sf]; sd.s1 = a.faces[3 * (size_t)sf + 1]; sd.s2 = a.faces[3 * (size_t)sf + 2]; sd.noexpand = 0;
-    float sdist[3];
-    {
-      const uint32_t sv[3] = {sd.s0, sd.s1, sd.s2};
-      for (int k = 0; k < 3; ++k) {   // cvp:719-728
-        const float dx = a.seed_pos[3 * (size_t)q] - a.pos[3 * (size_t)sv[k]];
-        const float dy = a.seed_pos[3 * (size_t)q + 1] - a.pos[3 * (size_t)sv[k] + 1];
-        const float dz = a.seed_pos[3 * (size_t)q + 2] - a.pos[3 * (size_t)sv[k] + 2];
-        sdist[k] = sqrtf(dx * dx + dy * dy + dz * dz);
-        if (((double)a.cost[sv[k]] >= a.cost_limit) || (a.invalid && a.invalid[sv[k]])) sd.noexpand |= (1u << k);  // cvp:757,760
-      }
-    }
-    const float seed_min = fminf(sdist[0], fminf(sdist[1], sdist[2]));
-    sd.seed_max = fmaxf(sdist[0], fmaxf(sdist[1], sdist[2]));
+    const CvpSeeds cs = cvp_seeds(a.faces, a.pos, a.cost, a.invalid, a.cost_limit, a.seed_faces[q], a.seed_pos + 3 * (size_t)q);
+    const SeedFace sd = cs;
     if (gtid == 0) {
-      const uint32_t sv[3] = {sd.s0, sd.s1, sd.s2};
-      for (int k = 0; k < 3; ++k) {
-        G.state[sv[k]] = make_uint4(__float_as_uint(sdist[k]), __float_as_uint(sdist[k]), 0u, 0u);
-        G.mark[sv[k]] = MARK_FIXED;
-      }
+      for (int k = 0; k < 3; ++k) { put_seed_label(G.state[cs.s[k]], cs.d[k]); G.mark[cs.s[k]] = MARK_FIXED; }
       unsigned int n0 = 0;
       for (int k = 0; k < 3; ++k) {
-        const uint32_t kb = a.cor_ptr[sv[k]], ke = a.cor_ptr[sv[k] + 1];
+        const uint32_t kb = a.cor_ptr[cs.s[k]], ke = a.cor_ptr[cs.s[k] + 1];
         for (uint32_t kk = kb; kk < ke; ++kk) {
           const int4 ix = a.cor_idx[kk];
           const uint32_t xs[2] = {(uint32_t)ix.x, (uint32_t)ix.y};
           for (int t = 0; t < 2; ++t) {
             const uint32_t x = xs[t];
+            // (CvpProblem::eligible written out: through the call k_cvp_batch<1, false> takes 16 bytes more stack)
             if (G.mark[x] == MARK_NONE && !(a.invalid && a.invalid[x]) && !((double)a.cost[x] >= a.cost_limit)) { G.mark[x] = MARK_CAND; list0[n0++] = x; }
           }
         }
       }
-      ctl_reset(ctl, n0, seed_min);
+      ctl_reset(ctl, n0, cs.seed_min);
       if constexpr (MATRIX) ctl->targets_left = (int)a.tg.distinct;
     }
     group_sync<CS>();
     if constexpr (MATRIX) {
-      count_targets_done_at_init(a.tg, ctl, G.mark, V, gthreads, gtid, [&](uint32_t v) {   // candidates: k_cvp_batch's activation test
-        return !(a.invalid && a.invalid[v]) && !((double)a.cost[v] >= a.cost_limit);
-      });
+      count_targets_done_at_init(a.tg, ctl, G.mark, V, gthreads, gtid,
+                                 [&](uint32_t v) { return CvpProblem::eligible(v, a.cost, a.invalid, a.cost_limit); });
       group_sync<CS>();
     }
     run_band_rounds_batch<CS, MATRIX>(a, G, list0, list1, st, wk, a.delta, gthreads, gtid, sd, nextafterf(sd.seed_max, __uint_as_float(INF_BITS)));
@@ -376,79 +348,23 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
   __shared__ SweepStage sws;
   uint32_t g, gthreads, gtid;
   group_coords<0>(g, gthreads, gtid);
-  const uint32_t V = a.V;
-  uint4* state = a.ws.state; uint32_t* mark = a.ws.mark; uint32_t* list0 = a.ws.list0; uint32_t* list1 = a.ws.list1;
   GroupCtl* ctl = a.ws.ctl;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; sws.dn[0] = 0; sws.dn[1] = 0; }
+  if (threadIdx.x == 0) { stage_init(st); sws.dn[0] = 0; sws.dn[1] = 0; }
   __syncthreads();
-  if constexpr (!RESUME) {
-    for (uint32_t v = gtid; v < V; v += gthreads) { state[v] = state_inf(); mark[v] = MARK_NONE; a.ws.chg[v] = 0u; a.ws.ver[v] = 0u; }
-    group_sync<0>(ctl->barrier);
-  }
-  const uint32_t sf = a.seed_faces[0];
-  const uint32_t s0 = a.faces[3 * (size_t)sf], s1 = a.faces[3 * (size_t)sf + 1], s2 = a.faces[3 * (size_t)sf + 2];
   CvpEllProblem prob;
-  prob.cor_ptr = a.cor_ptr; prob.cor_idx = a.cor_idx; prob.cor_w = a.cor_w; prob.cost = a.cost; prob.invalid = a.invalid;
-  prob.ell_idx = a.ell_idx; prob.ell_w = a.ell_w; prob.ell_geo = a.ell_geo;
-  prob.state = state; prob.ext_arr = a.ws.ext; prob.root_arr = a.ws.root; prob.chg = a.ws.chg;
-  prob.pool_w = a.ws.pool; prob.pool = prob.pool_w; prob.pool_cap = a.ws.pool_cap; prob.pool_top = &ctl->pool_top; prob.pool_overflow = &ctl->pool_overflow;
-  prob.ver = a.ws.ver; prob.deferred_m = __uint_as_float(INF_BITS); prob.pred = nullptr; prob.dir = nullptr; prob.cut = nullptr; prob.cost_limit = a.cost_limit;
-  prob.s0 = s0; prob.s1 = s1; prob.s2 = s2; prob.seed_noexpand = 0; prob.goal_t = ev_normal(__uint_as_float(INF_BITS), 0u);
-  prob.prefetch_marks = true;
-  float sd[3];
-  {
-    const uint32_t sv[3] = {s0, s1, s2};
-    for (int k = 0; k < 3; ++k) {   // cvp:719-728
-      const float dx = a.seed_pos[0] - a.pos[3 * (size_t)sv[k]];
-      const float dy = a.seed_pos[1] - a.pos[3 * (size_t)sv[k] + 1];
-      const float dz = a.seed_pos[2] - a.pos[3 * (size_t)sv[k] + 2];
-      sd[k] = sqrtf(dx * dx + dy * dy + dz * dz);
-      const bool noexp = ((double)a.cost[sv[k]] >= a.cost_limit) || (a.invalid && a.invalid[sv[k]]);
-      if (noexp) prob.seed_noexpand |= (1u << k);
-    }
-  }
-  const float seed_min = fminf(sd[0], fminf(sd[1], sd[2]));
-  const float seed_max = fmaxf(sd[0], fmaxf(sd[1], sd[2]));
-  prob.seed_max_d = seed_max;
-  uint32_t r0 = 0xffffffffu, r1 = 0xffffffffu, r2 = 0xffffffffu;
-  const int has_robot = a.robot_face >= 0;
-  if (has_robot) {
-    r0 = a.faces[3 * (size_t)a.robot_face]; r1 = a.faces[3 * (size_t)a.robot_face + 1]; r2 = a.faces[3 * (size_t)a.robot_face + 2];
-  }
-  if (gtid == 0) {
-    const uint32_t sv[3] = {s0, s1, s2};
-    if constexpr (!RESUME) {
-      for (int k = 0; k < 3; ++k) { state[sv[k]] = make_uint4(__float_as_uint(sd[k]), __float_as_uint(sd[k]), 0u, 0u); mark[sv[k]] = MARK_FIXED; }
-      unsigned int n0 = 0;
-      for (int k = 0; k < 3; ++k)
-        prob.activate(sv[k], [&](uint32_t x) {
-          if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-        });
-      ctl_reset(ctl, n0, seed_min);
-    }
-    if (has_robot) {
-      int left = 0; const uint32_t rv[3] = {r0, r1, r2};
-      for (int k = 0; k < 3; ++k) if (mark[rv[k]] != MARK_FIXED) left++;
-      ctl->robot_left = left;
-      if (left == 0) {
-        ctl->goal_ring[0] = __float_as_uint((float)((double)seed_max + a.goal_dist_offset));
-        uint32_t sl = sv[0]; float sdl = sd[0];
-        for (int k = 1; k < 3; ++k) if (sd[k] > sdl || (sd[k] == sdl && sv[k] > sl)) { sl = sv[k]; sdl = sd[k]; }
-        ctl->goal_time[0] = __float_as_uint(sdl); ctl->goal_time[1] = sl; ctl->goal_time[5] = sl;
-      }
-    }
-  }
-  group_sync<0>(ctl->barrier);
+  uint32_t rv[3];
+  cvp_single_setup<0, RESUME>(a, true, true, gthreads, gtid, prob, rv);
   const float delta = a.delta;      // not clamped to goal_dist_offset: the engine caps settling instead (settle_cap)
   // in-round sweeps pay off once the band is several dependency hops deep; 12 were measured best on the 5M terrain
   int sweeps = a.sweeps;
   if (sweeps < 0) sweeps = delta < 2.8f * a.hop ? 0 : min(12, (int)(delta / a.hop));
-  const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : seed_max;    // (see k_cvp)
-  run_band_rounds_sub8<0, true, CvpEllProblem, RESUME>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, r0, r1, r2,
-                          a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)), a.max_rounds, sweeps, &sws, V);
+  const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : prob.seed_max_d;    // (see k_cvp)
+  run_band_rounds_sub8<0, true, CvpEllProblem, RESUME>(prob, ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, a.robot_face >= 0,
+                          rv[0], rv[1], rv[2], a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)), a.max_rounds,
+                          sweeps, &sws, a.V);
   group_sync<0>(ctl->barrier);
   if (a.out_dist)
-    for (uint32_t v = gtid; v < V; v += gthreads) a.out_dist[v] = __uint_as_float(state[v].x);
+    for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
 }
 
 // the epilogue of a single plan (cvp_epilogue_problem above), one thread per vertex; the goal cutoff is the plan's
@@ -456,11 +372,9 @@ __global__ void __launch_bounds__(256) k_cvp_epilogue(const CvpKernelArgs a, Gro
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= a.V) return;
   const uint32_t sf = a.seed_faces[0];
-  EvTime goal_t;
-  goal_t.a1 = __uint_as_float(ctl->goal_time[0]); goal_t.root = ctl->goal_time[1]; goal_t.a2 = __uint_as_float(ctl->goal_time[2]);
-  goal_t.a3 = __uint_as_float(ctl->goal_time[3]); goal_t.ext = ctl->goal_time[4]; goal_t.self = ctl->goal_time[5];
   CvpProblem prob;
-  cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, goal_t, a.out_pred, a.out_dir, a.out_cut, prob);
+  cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, a.seed_pos, time_get(ctl->goal_time),
+                       a.out_pred, a.out_dir, a.out_cut, prob);
   cvp_epilogue_vertex(prob, ctl, sf, __uint_as_float(ctl->goal_bits), c);
 }
 
@@ -484,18 +398,6 @@ struct ReplanArgs {
   uint32_t* t0;                     // [8 + 6 * blocks of k_replan_t0]: T0, the resume flag, one spare word, the block minima
 };
 constexpr uint32_t REPLAN_T0_WORDS = 8;
-
-// a pop time as six words, in the order of GroupCtl::goal_time: a1 bits, root, a2 bits, a3 bits, ext, vertex
-__device__ __forceinline__ void time_put(uint32_t* w, const EvTime& t) {
-  w[0] = __float_as_uint(t.a1); w[1] = t.root; w[2] = __float_as_uint(t.a2); w[3] = __float_as_uint(t.a3); w[4] = t.ext; w[5] = t.self;
-}
-__device__ __forceinline__ EvTime time_get(const uint32_t* w) {
-  EvTime t; t.a1 = __uint_as_float(__ldcg(&w[0])); t.root = __ldcg(&w[1]); t.a2 = __uint_as_float(__ldcg(&w[2]));
-  t.a3 = __uint_as_float(__ldcg(&w[3])); t.ext = __ldcg(&w[4]); t.self = __ldcg(&w[5]);
-  return t;
-}
-// later than every finite pop time
-__device__ __forceinline__ EvTime time_never() { return ev_normal(__uint_as_float(INF_BITS), 0xffffffffu); }
 
 __device__ __forceinline__ LabelStore replan_store(const ReplanArgs& a) {
   LabelStore s;
@@ -625,7 +527,7 @@ __global__ void __launch_bounds__(256) k_replan_frontier(const ReplanArgs a) {
   }
 #endif
   if (mv != MARK_NONE) return;
-  if ((a.invalid && a.invalid[v]) || (double)a.cost[v] >= a.cost_limit) return;
+  if (!CvpProblem::eligible(v, a.cost, a.invalid, a.cost_limit)) return;
   bool next_to_kept = false;
   for (uint32_t k = __ldg(&a.cor_ptr[v]), ke = __ldg(&a.cor_ptr[v + 1]); k < ke && !next_to_kept; ++k) {
     const int4 ix = __ldg(&a.cor_idx[k]);
@@ -659,41 +561,44 @@ struct DijkstraKernelArgs {
   const uint4* ell_adj; int sweeps; float hop;   // whole-grid kernel only
 };
 
+// The prologue of a single-plan Dijkstra wave (k_dijkstra, k_dijkstra_grid): the clearing pass (the sweep versions only for
+// the kernel with in-round sweeps), the problem, the seed (dijkstra:276, d = 0) with its first candidates, and the robot
+// vertex still to settle.  Called by every thread of the group; ends with a group barrier.
+template <int CS>
+__device__ __forceinline__ void dijkstra_single_setup(const DijkstraKernelArgs& a, bool clear_ver, uint32_t gthreads, uint32_t gtid,
+                                                      DijkstraProblem& prob) {
+  for (uint32_t v = gtid; v < a.V; v += gthreads) {
+    a.ws.state[v] = state_inf(); a.ws.mark[v] = MARK_NONE; a.out_pred[v] = v;
+    if (clear_ver) a.ws.ver[v] = 0u;
+  }
+  group_sync<CS>();
+  prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
+  prob.state = a.ws.state; prob.pred = a.out_pred; prob.cost_limit = a.cost_limit; prob.deferred_m = __uint_as_float(INF_BITS); prob.strict = 0;
+  if (gtid == 0) {
+    const float d0 = 0.0f;
+    seed_wave(prob, a.ws.ctl, a.ws.mark, a.ws.list0, &a.seed_vertex, &d0, 1, 0.0f);
+    if (a.robot_vertex >= 0) a.ws.ctl->robot_left = 1;
+  }
+  group_sync<CS>();
+}
+
 template <int CS>
 __global__ void __launch_bounds__(512, 1) k_dijkstra(const DijkstraKernelArgs a) {
   __shared__ Stage st;
   uint32_t g, gthreads, gtid;
   group_coords<CS>(g, gthreads, gtid);
-  const uint32_t V = a.V;
-  uint4* state = a.ws.state;
-  uint32_t* mark = a.ws.mark; uint32_t* list0 = a.ws.list0; uint32_t* list1 = a.ws.list1;
-  GroupCtl* ctl = a.ws.ctl;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  if (threadIdx.x == 0) stage_init(st);
   __syncthreads();
-  for (uint32_t v = gtid; v < V; v += gthreads) { state[v] = state_inf(); mark[v] = MARK_NONE; a.out_pred[v] = v; }
-  group_sync<CS>(ctl->barrier);
   DijkstraProblem prob;
-  prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
-  prob.state = state; prob.pred = a.out_pred; prob.cost_limit = a.cost_limit; prob.deferred_m = __uint_as_float(INF_BITS);
+  dijkstra_single_setup<CS>(a, false, gthreads, gtid, prob);
   const int has_robot = a.robot_vertex >= 0;
   const uint32_t rv = has_robot ? (uint32_t)a.robot_vertex : 0xffffffffu;
-  if (gtid == 0) {
-    state[a.seed_vertex] = make_uint4(0u, 0u, 0u, 0u);     // dijkstra:276 (d = 0, tau = 0)
-    mark[a.seed_vertex] = MARK_FIXED;
-    unsigned int n0 = 0;
-    prob.activate(a.seed_vertex, [&](uint32_t x) {
-      if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-    });
-    ctl_reset(ctl, n0, 0.0f);
-    if (has_robot) ctl->robot_left = 1;
-  }
-  group_sync<CS>();
   float delta = a.delta;
   if (has_robot && a.goal_dist_offset < (double)delta) delta = (float)fmax(a.goal_dist_offset, 1e-4);
-  run_band_rounds<CS>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, rv, rv, rv,
+  run_band_rounds<CS>(prob, a.ws.ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, has_robot, rv, rv, rv,
                       a.goal_dist_offset, a.cancel_flag, 1e-30f, a.max_rounds);
   group_sync<CS>();
-  for (uint32_t v = gtid; v < V; v += gthreads) a.out_dist[v] = __uint_as_float(state[v].x);
+  for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
 }
 
 // Batches of full-field Dijkstra plans (mnb_dijkstra_batch): the outer loop of k_cvp_batch around the round loop of
@@ -741,7 +646,7 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijk
   uint32_t* list1 = a.ws.list1 + (size_t)g * V;
   GroupCtl* ctl = a.ws.ctl + g;
   const volatile int* cancel = a.cancel_flag;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  if (threadIdx.x == 0) stage_init(st);
   __syncthreads();
   DijkstraProblemT<float> prob;
   prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
@@ -758,15 +663,9 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijk
     }
     group_sync<CS>();
     prob.pred = pred;
-    const uint32_t s = a.seeds[q];
     if (gtid == 0) {
-      label[s] = 0.0f;                                         // dijkstra:276
-      mark[s] = MARK_FIXED;
-      unsigned int n0 = 0;
-      prob.activate(s, [&](uint32_t x) {
-        if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-      });
-      ctl_reset(ctl, n0, 0.0f);
+      const float d0 = 0.0f;                                   // dijkstra:276
+      seed_wave(prob, ctl, mark, list0, &a.seeds[q], &d0, 1, 0.0f);
       if constexpr (MATRIX) ctl->targets_left = (int)a.tg.distinct;
     }
     group_sync<CS>();
@@ -826,7 +725,7 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijk
   uint32_t* list1 = a.ws.list1 + (size_t)g * V;
   GroupCtl* ctl = a.ws.ctl + g;
   const volatile int* cancel = a.cancel_flag;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; }
+  if (threadIdx.x == 0) stage_init(st);
   __syncthreads();
   DijkstraRepairProblem prob;
   prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
@@ -937,36 +836,18 @@ __global__ void __launch_bounds__(512, 1) k_dijkstra_grid(const DijkstraKernelAr
   __shared__ SweepStage sws;
   uint32_t g, gthreads, gtid;
   group_coords<0>(g, gthreads, gtid);
-  const uint32_t V = a.V;
-  uint4* state = a.ws.state;
-  uint32_t* mark = a.ws.mark; uint32_t* list0 = a.ws.list0; uint32_t* list1 = a.ws.list1;
-  GroupCtl* ctl = a.ws.ctl;
-  if (threadIdx.x == 0) { st.n = 0; st.m_tau = INF_BITS; st.lo = INF_BITS; sws.dn[0] = 0; sws.dn[1] = 0; }
+  if (threadIdx.x == 0) { stage_init(st); sws.dn[0] = 0; sws.dn[1] = 0; }
   __syncthreads();
-  for (uint32_t v = gtid; v < V; v += gthreads) { state[v] = state_inf(); mark[v] = MARK_NONE; a.out_pred[v] = v; a.ws.ver[v] = 0u; }
-  group_sync<0>(ctl->barrier);
   DijkstraEllProblem prob;
-  prob.adj_ptr = a.adj_ptr; prob.adj_nw = a.adj_nw; prob.cost = a.cost; prob.invalid = a.invalid;
-  prob.state = state; prob.pred = a.out_pred; prob.cost_limit = a.cost_limit; prob.deferred_m = __uint_as_float(INF_BITS);
-  prob.strict = 0; prob.ell_adj = a.ell_adj; prob.ver = a.ws.ver;
+  dijkstra_single_setup<0>(a, true, gthreads, gtid, prob);
+  prob.ell_adj = a.ell_adj; prob.ver = a.ws.ver;
   const int has_robot = a.robot_vertex >= 0;
   const uint32_t rv = has_robot ? (uint32_t)a.robot_vertex : 0xffffffffu;
-  if (gtid == 0) {
-    state[a.seed_vertex] = make_uint4(0u, 0u, 0u, 0u);     // dijkstra:276 (d = 0, tau = 0)
-    mark[a.seed_vertex] = MARK_FIXED;
-    unsigned int n0 = 0;
-    prob.activate(a.seed_vertex, [&](uint32_t x) {
-      if (mark[x] == MARK_NONE && prob.eligible(x)) { mark[x] = MARK_CAND; list0[n0++] = x; }
-    });
-    ctl_reset(ctl, n0, 0.0f);
-    if (has_robot) ctl->robot_left = 1;
-  }
-  group_sync<0>(ctl->barrier);
   const float delta = a.delta;      // not clamped to goal_dist_offset: the engine caps settling instead (settle_cap)
   int sweeps = a.sweeps;
   if (sweeps < 0) sweeps = delta < 2.8f * a.hop ? 0 : min(15, (int)(delta / a.hop));
-  run_band_rounds_sub8<0, true>(prob, ctl, list0, list1, mark, st, delta, gthreads, gtid, has_robot, rv, rv, rv,
-                                a.goal_dist_offset, a.cancel_flag, 1e-30f, a.max_rounds, sweeps, &sws, V);
-  group_sync<0>(ctl->barrier);
-  for (uint32_t v = gtid; v < V; v += gthreads) a.out_dist[v] = __uint_as_float(state[v].x);
+  run_band_rounds_sub8<0, true>(prob, a.ws.ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, has_robot, rv, rv, rv,
+                                a.goal_dist_offset, a.cancel_flag, 1e-30f, a.max_rounds, sweeps, &sws, a.V);
+  group_sync<0>(a.ws.ctl->barrier);
+  for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
 }

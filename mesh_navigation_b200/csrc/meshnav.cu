@@ -881,8 +881,6 @@ static int32_t launch_single_cvp(mnb_ctx* ctx, CvpKernelArgs a) {
     }
     CK(launch_cooperative(k_cvp_grid<RESUME>, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
   } else {
-    // k_cvp takes its query from the counter and bumps it again to leave its loop: every launch starts from zero
-    CK(cudaMemsetAsync(a.next_query, 0, sizeof(unsigned int), ctx->stream));
     const cudaError_t e = with_cluster_size<16>(ctx->cluster, [&](auto c) {
       constexpr int CS = decltype(c)::value;
       return launch_cluster(k_cvp<CS, RESUME>, a, CS, (unsigned)CS, MNB_CVP_THREADS, ctx->stream);

@@ -55,10 +55,11 @@ struct CvpProblem : LabelStore {
     deferred_m = fminf(deferred_m, T.a1);
     return false;
   }
-  __device__ __forceinline__ bool eligible(uint32_t x) const {
+  __device__ __forceinline__ static bool eligible(uint32_t x, const float* cost, const uint8_t* invalid, double cost_limit) {
     if (invalid && invalid[x]) return false;        // cvp:785 (no face with an invalid vertex)
     return !((double)cost[x] >= cost_limit);        // cvp:802,825,848
   }
+  __device__ __forceinline__ bool eligible(uint32_t x) const { return eligible(x, cost, invalid, cost_limit); }
   __device__ __forceinline__ static bool never_fixed(uint32_t) { return false; }
   __device__ __forceinline__ int seed_index(uint32_t v) const { return v == s0 ? 0 : (v == s1 ? 1 : (v == s2 ? 2 : -1)); }
 
@@ -201,6 +202,30 @@ struct CvpProblem : LabelStore {
     return true;
   }
 };
+
+// The seed face of a CVP wave as the problem reads it: its vertices s0-s2, the seeds that pop but do not expand (bit k: seed
+// k, cvp:757,760) and the largest seed potential
+struct SeedFace { uint32_t s[3]; uint32_t noexpand; float seed_max; };
+// ... and what the seeding writes: the seed potentials, the distances of the vertices to the seed point (cvp:719-728)
+struct CvpSeeds : SeedFace { float d[3]; float seed_min; };
+// the seed face sf with seed point sp
+__device__ __forceinline__ CvpSeeds cvp_seeds(const uint32_t* faces, const float* pos, const float* cost, const uint8_t* invalid,
+                                              double cost_limit, uint32_t sf, const float* sp) {
+  CvpSeeds sd;
+  sd.noexpand = 0;
+  for (int k = 0; k < 3; ++k) {
+    const uint32_t v = faces[3 * (size_t)sf + k];
+    const float dx = sp[0] - pos[3 * (size_t)v];
+    const float dy = sp[1] - pos[3 * (size_t)v + 1];
+    const float dz = sp[2] - pos[3 * (size_t)v + 2];
+    sd.s[k] = v;
+    sd.d[k] = sqrtf(dx * dx + dy * dy + dz * dz);
+    if (((double)cost[v] >= cost_limit) || (invalid && invalid[v])) sd.noexpand |= (1u << k);
+  }
+  sd.seed_min = fminf(sd.d[0], fminf(sd.d[1], sd.d[2]));
+  sd.seed_max = fmaxf(sd.d[0], fmaxf(sd.d[1], sd.d[2]));
+  return sd;
+}
 
 // ---------------------------------------------------------------------------
 // CVP, 8 lanes per candidate ("sub-warp pull").  Corner records live in an ELL
