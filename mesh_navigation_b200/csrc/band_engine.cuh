@@ -319,6 +319,7 @@ struct GroupCtl {               // one per wavefront group, global memory
   // discipline: round r reads slot r&1, the thread that settles the last target in round r raises slot (r+1)&1.
   int targets_left;
   unsigned int done_ring[2];
+  unsigned int epi_csr;         // k_cvp_epilogue: vertices it listed for the CSR replay of k_cvp_epilogue_csr
 };
 
 // a pop time as six words, in the order of GroupCtl::goal_time: a1 bits, root, a2 bits, a3 bits, ext, vertex

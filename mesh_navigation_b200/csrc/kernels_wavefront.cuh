@@ -233,8 +233,20 @@ __device__ __forceinline__ void cvp_epilogue_problem(const CvpKernelArgs& a, uin
   cvp_problem(a, state, ext, root, chg, pool, a.ws.pool_cap, ctl, sd, goal_t, pred, dir, cut, prob);
 }
 
-// one vertex c of the epilogue (goal: the goal cutoff's potential, +inf when not armed)
-__device__ __forceinline__ void cvp_epilogue_vertex(CvpProblem& prob, GroupCtl* ctl, uint32_t sf, float goal, uint32_t c) {
+// one vertex c of the epilogue (goal: the goal cutoff's potential, +inf when not armed).  ROW: the replay runs on c's ELL
+// row in registers (CvpProblem::replay_row), and a vertex it does not cover (more than 8 faces, a cascade member among the
+// sources) is handed to csr(c), which runs CvpProblem::epilogue_csr -- at once or in a launch of its own.  !ROW: the CSR
+// replay in line, for a caller whose registers cannot hold a row: at the 64 registers of the batch kernels the row
+// replay spills, and the batch with fields was measured 13 % slower with it.
+template <bool ROW, class Csr>
+__device__ __forceinline__ void cvp_epilogue_vertex(CvpProblem& prob, const int4* __restrict__ ell_idx, const float4* __restrict__ ell_w,
+                                                    GroupCtl* ctl, uint32_t sf, float goal, uint32_t c, Csr csr) {
+  const int4* row = ell_idx + (size_t)c * ELL_W;
+  int4 ix[ELL_W];                                        // (requested together with the label of c)
+  if constexpr (ROW) {
+#pragma unroll
+    for (int j = 0; j < (int)ELL_W; ++j) ix[j] = __ldg(&row[j]);
+  }
   const uint4 lw = __ldcg(&prob.state[c]);
   const float d = __uint_as_float(lw.x);
   // statistic: labels whose pop time has more than 3 cascade levels (their tails live in the level pool; exact)
@@ -245,10 +257,21 @@ __device__ __forceinline__ void cvp_epilogue_vertex(CvpProblem& prob, GroupCtl* 
     if (prob.cut) prob.cut[c] = (int32_t)sf;
     return;
   }
-  int win = -1; float nd, wu1 = 0, wu2 = 0; EvFull nt;
-  if (__float_as_uint(d) != INF_BITS && prob.eligible(c))
-    prob.replay(c, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, nd, nt, win, wu1, wu2);
-  prob.write_aux(c, win, wu1, wu2);
+  if constexpr (!ROW) {
+    int win = -1; float nd, wu1 = 0, wu2 = 0; EvFull nt;
+    if (__float_as_uint(d) != INF_BITS && prob.eligible(c))
+      prob.replay(c, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, nd, nt, win, wu1, wu2);
+    prob.write_aux(c, win, wu1, wu2);
+  } else {
+    if (__float_as_uint(d) == INF_BITS || !prob.eligible(c)) { prob.write_aux_none(c); return; }
+    int win; float4 ww; float wu1, wu2;
+    if (!prob.replay_row(c, ix, ell_w, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, win, ww, wu1, wu2)) {
+      csr(c);
+      return;
+    }
+    if (win < 0) prob.write_aux_none(c);
+    else prob.write_aux(c, __ldg(&row[win]), ww, wu1, wu2);
+  }
 }
 
 // k_cvp_batch<CS, true>: the epilogue of goal q over the group's workspace, rows q of out_pred / out_dir / out_cut (each may
@@ -260,7 +283,7 @@ __device__ __noinline__ void batch_fields_epilogue(const CvpKernelArgs& a, const
   CvpProblem prob;
   cvp_epilogue_problem(a, G.state, G.ext_arr, G.root_arr, G.chg, G.pool, G.ctl, sf, a.seed_pos + 3 * (size_t)q, ev_normal(__uint_as_float(INF_BITS), 0u),
                        a.out_pred ? a.out_pred + row : nullptr, a.out_dir ? a.out_dir + row : nullptr, a.out_cut ? a.out_cut + row : nullptr, prob);
-  for (uint32_t v = gtid; v < V; v += gthreads) cvp_epilogue_vertex(prob, G.ctl, sf, __uint_as_float(INF_BITS), v);
+  for (uint32_t v = gtid; v < V; v += gthreads) cvp_epilogue_vertex<false>(prob, a.ell_idx, a.ell_w, G.ctl, sf, __uint_as_float(INF_BITS), v, [](uint32_t) {});
 }
 
 // FIELDS = false: potentials only (mnb_cvp_batch, and mnb_cvp_batch_fields asked for potentials alone).  FIELDS = true:
@@ -367,15 +390,32 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
     for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
 }
 
-// the epilogue of a single plan (cvp_epilogue_problem above), one thread per vertex; the goal cutoff is the plan's
-__global__ void __launch_bounds__(256) k_cvp_epilogue(const CvpKernelArgs a, GroupCtl* ctl) {
+// The epilogue of a single plan (cvp_epilogue_problem above), one thread per vertex; the goal cutoff is the plan's.  In two
+// launches: k_cvp_epilogue replays every vertex its ELL row covers, in registers, and lists the others (ws.list1, free once
+// the wave has ended; ctl->epi_csr entries, cleared by the host before the launch); k_cvp_epilogue_csr replays those on
+// their CSR records.  A call to the out-of-line replay would cost the first kernel its registers: the call convention
+// caps them and saves the live ones to a stack frame.
+#ifndef MNB_EPILOGUE_THREADS
+#define MNB_EPILOGUE_THREADS 256
+#endif
+__global__ void __launch_bounds__(MNB_EPILOGUE_THREADS) k_cvp_epilogue(const CvpKernelArgs a, GroupCtl* ctl) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= a.V) return;
   const uint32_t sf = a.seed_faces[0];
   CvpProblem prob;
   cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, a.seed_pos, time_get(ctl->goal_time),
                        a.out_pred, a.out_dir, a.out_cut, prob);
-  cvp_epilogue_vertex(prob, ctl, sf, __uint_as_float(ctl->goal_bits), c);
+  cvp_epilogue_vertex<true>(prob, a.ell_idx, a.ell_w, ctl, sf, __uint_as_float(ctl->goal_bits), c,
+                      [&](uint32_t v) { a.ws.list1[atomicAdd(&ctl->epi_csr, 1u)] = v; });
+}
+__global__ void __launch_bounds__(256) k_cvp_epilogue_csr(const CvpKernelArgs a, GroupCtl* ctl) {
+  const uint32_t n = __ldcg(&ctl->epi_csr);
+  const uint32_t sf = a.seed_faces[0];
+  CvpProblem prob;
+  cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, a.seed_pos, time_get(ctl->goal_time),
+                       a.out_pred, a.out_dir, a.out_cut, prob);
+  const float goal = __uint_as_float(ctl->goal_bits);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) prob.epilogue_csr(__ldcg(&a.ws.list1[i]), goal);
 }
 
 // ============================================================================

@@ -18,9 +18,11 @@ static inline cudaError_t mnb_interpreted_launch(void (*kern)(KArgs...), unsigne
 #define MNB_DYNAMIC_SMEM(name) extern __shared__ __align__(16) unsigned char name[]
 #endif
 
-// fire-and-forget prefetch of the line at p into the L2 (no register, no scoreboard); a no-op on the CPU interpreter
+// fire-and-forget prefetch of the line at p into the L2 / the L1 (no register, no scoreboard); no-ops on the CPU interpreter
 #ifdef MNB_EMU_ACTIVE
 static inline void mnb_prefetch_l2(const void*) {}
+static inline void mnb_prefetch_l1(const void*) {}
 #else
 __device__ __forceinline__ void mnb_prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+__device__ __forceinline__ void mnb_prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 #endif

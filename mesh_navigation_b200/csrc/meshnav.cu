@@ -868,7 +868,8 @@ static void fill_cvp_args(mnb_ctx* ctx, CvpKernelArgs& a) {
 }
 
 // A single plan's wave on the workspace of a.ws: k_cvp_grid or, with mnb_set_tuning(cluster >= 1), k_cvp<CS> -- in the
-// resumed form with RESUME (mnb_cvp_replan) -- then the epilogue.
+// resumed form with RESUME (mnb_cvp_replan) -- then the epilogue (k_cvp_epilogue, k_cvp_epilogue_csr).
+constexpr unsigned SINGLE_CVP_LAUNCHES = 3;
 template <bool RESUME>
 static int32_t launch_single_cvp(mnb_ctx* ctx, CvpKernelArgs a) {
   if (ctx->cluster == -1) {
@@ -887,7 +888,9 @@ static int32_t launch_single_cvp(mnb_ctx* ctx, CvpKernelArgs a) {
     });
     if (e != cudaSuccess) { ctx->err = std::string("cvp launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   }
-  MNB_LAUNCH(k_cvp_epilogue, (ctx->V + 255) / 256, 256, 0, ctx->stream, a, a.ws.ctl);
+  CK(cudaMemsetAsync(&a.ws.ctl->epi_csr, 0, sizeof(unsigned int), ctx->stream));
+  MNB_LAUNCH(k_cvp_epilogue, (ctx->V + MNB_EPILOGUE_THREADS - 1) / MNB_EPILOGUE_THREADS, MNB_EPILOGUE_THREADS, 0, ctx->stream, a, a.ws.ctl);
+  MNB_LAUNCH(k_cvp_epilogue_csr, (unsigned)(4 * ctx->sm_count), 256, 0, ctx->stream, a, a.ws.ctl);   // (grid-stride over the list)
   CK(cudaGetLastError());
   return MNB_OK;
 }
@@ -951,7 +954,7 @@ static int32_t impl_cvp(mnb_ctx* ctx, uint32_t seed_face, const float seed_pos[3
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
   if ((rc = launch_single_cvp<false>(ctx, a)) != MNB_OK) return rc;
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
-  return single_cvp_outcome(ctx, a, io, seed_face, seed_pos, robot_face, 2);
+  return single_cvp_outcome(ctx, a, io, seed_face, seed_pos, robot_face, SINGLE_CVP_LAUNCHES);
 }
 
 // mnb_cvp_replan: the arguments of mnb_cvp plus the union of the changed sets of the mnb_update_vertex_costs calls since
@@ -1023,7 +1026,7 @@ static int32_t impl_cvp_replan(mnb_ctx* ctx, uint32_t seed_face, const float see
       CvpKernelArgs ra = a;
       if (ctx->replan_pool_room) ra.ws.pool_cap = std::min<uint32_t>(ra.ws.pool_cap, ctx->rw_pool_top + ctx->replan_pool_room);
       if ((rc = launch_single_cvp<true>(ctx, ra)) != MNB_OK) return rc;
-      launches += 4;
+      launches += 2 + SINGLE_CVP_LAUNCHES;
       // the resumed wave allocates behind the old records: if the pool ran out, the whole wave starts from an empty one
       unsigned int overflow = 0;
       CK(cudaMemcpyAsync(&overflow, &a.ws.ctl->pool_overflow, sizeof(overflow), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1034,7 +1037,7 @@ static int32_t impl_cvp_replan(mnb_ctx* ctx, uint32_t seed_face, const float see
   if (!resume) {
     CK(cudaMemsetAsync(a.ws.ctl, 0, sizeof(GroupCtl), ctx->stream));
     if ((rc = launch_single_cvp<false>(ctx, a)) != MNB_OK) return rc;
-    launches += 2;
+    launches += SINGLE_CVP_LAUNCHES;
   }
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   rc = single_cvp_outcome(ctx, a, io, seed_face, seed_pos, robot_face, launches);

@@ -2,6 +2,7 @@
 #pragma once
 #include <type_traits>
 #include "band_engine.cuh"
+#include "launch.cuh"
 
 namespace mnb {
 
@@ -76,7 +77,10 @@ struct CvpProblem : LabelStore {
   // does the vertex with label L expand when it pops?  cvp:754: not if it lies beyond goal_dist -- the goal_dist of the
   // moment it pops: a vertex that popped before the cutoff was armed expanded whatever its potential
   __device__ __forceinline__ bool expands(const Label& L, float goal) const { return !(L.d > goal && !tless(L.t, goal_t)); }
-  // pop time T of the face with sources v1, v2 (= the pop of Tv); false if the face cannot fire
+  // pop time T of the face with sources v1, v2 (= the pop of Tv); false if the face cannot fire.  PLAIN: a and b are one-level
+  // times (ev_normal); the later source is then selected by value, so that its constant upper levels fold away (through a
+  // reference to one of the two, they stay in memory, and so do the out-of-line comparisons they would need)
+  template <bool PLAIN = false>
   __device__ __forceinline__ bool face_time(uint32_t c, uint32_t v1, uint32_t v2, const Label& a, const Label& b, float band_end,
                                             float goal, EvTime& T, uint32_t& Tv) const {
     if (!(a.d < band_end) || !(b.d < band_end)) return false;
@@ -98,7 +102,7 @@ struct CvpProblem : LabelStore {
         return !names(T, c);
       }
     }
-    const Label& L = v1_later ? a : b;                          // two normal sources: the later pop, if that vertex expands
+    std::conditional_t<PLAIN, const Label, const Label&> L = v1_later ? a : b;   // two normal sources: the later pop, if that vertex expands
     if (names(L.t, c)) return false;                            // the face fires inside a cascade of c itself (LabelStore::names)
     if (!expands(L, goal)) return false;
     T = L.t; Tv = v1_later ? v1 : v2;
@@ -112,21 +116,25 @@ struct CvpProblem : LabelStore {
     return face_time(c, (uint32_t)ix.x, (uint32_t)ix.y, a, b, band_end, goal, T, Tv);
   }
 
-  // predecessors_/direction_/cutting_faces_ of the winning face (cvp:493-517), literal acos form; a null output is skipped
+  // predecessors_/direction_/cutting_faces_ of the winning face (cvp:493-517), literal acos form; a null output is skipped.
+  // ix / w: the face's corner record and weights (a CSR record or the same entry of the ELL row)
+  __device__ __forceinline__ void write_aux(uint32_t c, const int4& ix, const float4& w, float wu1, float wu2) {
+    CvpResult r; r.value = 0; r.direction = 0; r.pred_sel = 1;
+    cvp_update_t<true>(wu1, wu2, (double)__uint_as_float(INF_BITS), w.z, w.y, w.x, r);
+    if (pred) pred[c] = r.pred_sel == 1 ? (uint32_t)ix.x : (uint32_t)ix.y;
+    if (dir) dir[c] = r.direction;
+    if (cut) cut[c] = ix.z;
+  }
+  // ... no face updated c (unreached, not eligible)
+  __device__ __forceinline__ void write_aux_none(uint32_t c) {
+    if (pred) pred[c] = c;
+    if (dir) dir[c] = 0.0f;
+    if (cut) cut[c] = -1;
+  }
+  // ... win: CSR corner record of the winning face, -1: none
   __device__ __forceinline__ void write_aux(uint32_t c, int win, float wu1, float wu2) {
-    if (win >= 0) {
-      const int4 ix = __ldg(&cor_idx[win]);
-      const float4 w = __ldg(&cor_w[win]);
-      CvpResult r; r.value = 0; r.direction = 0; r.pred_sel = 1;
-      cvp_update_t<true>(wu1, wu2, (double)__uint_as_float(INF_BITS), w.z, w.y, w.x, r);
-      if (pred) pred[c] = r.pred_sel == 1 ? (uint32_t)ix.x : (uint32_t)ix.y;
-      if (dir) dir[c] = r.direction;
-      if (cut) cut[c] = ix.z;
-    } else {
-      if (pred) pred[c] = c;
-      if (dir) dir[c] = 0.0f;
-      if (cut) cut[c] = -1;
-    }
+    if (win >= 0) write_aux(c, __ldg(&cor_idx[win]), __ldg(&cor_w[win]), wu1, wu2);
+    else write_aux_none(c);
   }
 
   // generic path for vertices with more than MAXF incident faces: repeated selection of the next
@@ -189,6 +197,86 @@ struct CvpProblem : LabelStore {
       if (cvp_update_t<false>(u1, u2, cur, w.z, w.y, w.x, r) && backstep_ok(r.value, T, Tv, round)) { cur = r.value; accept(c, r.value, T, tc); win = (int)k; wu1 = u1; wu2 = u2; }
     }
     nd = cur; nt = tc;
+  }
+
+  // replay() on the ELL row ix of c (slot j = corner cor_ptr[c] + j, ell_w laid out as cor_w), for the epilogue: the same
+  // face times, the same (T, corner) event order and the same accept loop, with every array index a compile-time constant
+  // so that the row, its source labels and the ranks stay in registers.  The event order comes from ranks (pairwise
+  // comparisons) instead of a sort.  Covered: at most 8 faces, and every source label word a plain one-level time (z = w
+  // = 0: no side arrays, no level pool), so that no comparison and no accept needs an out-of-line tail -- a plain trigger
+  // only ever hands out times of at most two levels.  Returns false for anything else (the caller runs replay()).
+  // win: winning slot (-1: none), with its weights ww and source potentials.
+  __device__ __forceinline__ bool replay_row(uint32_t c, const int4 (&ix)[ELL_W], const float4* __restrict__ ell_w, float band_end,
+                                             float goal, uint32_t round, int& win, float4& ww, float& wu1, float& wu2) const {
+    const float INF = __uint_as_float(INF_BITS);
+    if (ix[0].w > (int)ELL_W) return false;
+    // every load of the row first: its 16 source labels, and the line of its weights into L1 (read in the accept loop)
+    const float4* wrow = ell_w + (size_t)c * ELL_W;
+    mnb_prefetch_l1(wrow);
+    uint4 sa[ELL_W], sb[ELL_W];
+#pragma unroll
+    for (int j = 0; j < (int)ELL_W; ++j) {
+      sa[j] = state_inf(); sb[j] = state_inf();
+      if (ix[j].x != ELL_EMPTY) { sa[j] = __ldcg(&state[ix[j].x]); sb[j] = __ldcg(&state[ix[j].y]); }
+    }
+    uint32_t flags = 0u;
+#pragma unroll
+    for (int j = 0; j < (int)ELL_W; ++j) flags |= sa[j].z | sa[j].w | sb[j].z | sb[j].w;
+    if (flags) return false;                                       // a cascade member among the sources
+    // face times: (a1, Tv) of a plain pop time; a slot that does not fire sorts last
+    float A1[ELL_W], U1[ELL_W], U2[ELL_W]; uint32_t TV[ELL_W];
+    int n = 0;
+#pragma unroll
+    for (int j = 0; j < (int)ELL_W; ++j) {
+      A1[j] = INF; TV[j] = 0xffffffffu; U1[j] = 0.0f; U2[j] = 0.0f;
+      if (ix[j].x == ELL_EMPTY) continue;
+      const uint32_t v1 = (uint32_t)ix[j].x, v2 = (uint32_t)ix[j].y;
+      Label a, b;                                                  // = unpack_label() of a word with z = w = 0
+      a.d = __uint_as_float(sa[j].x); a.t = ev_normal(__uint_as_float(sa[j].y), v1);
+      b.d = __uint_as_float(sb[j].x); b.t = ev_normal(__uint_as_float(sb[j].y), v2);
+      EvTime T; uint32_t Tv;
+      if (!face_time<true>(c, v1, v2, a, b, band_end, goal, T, Tv)) continue;
+      A1[j] = T.a1; TV[j] = Tv; U1[j] = a.d; U2[j] = b.d; ++n;
+    }
+    // rank of slot j in (T, corner) order: for plain times tless is (a1, Tv), and equal times keep the corner order
+    int rank[ELL_W];
+#pragma unroll
+    for (int j = 0; j < (int)ELL_W; ++j) rank[j] = 0;
+#pragma unroll
+    for (int i = 0; i < (int)ELL_W; ++i)
+#pragma unroll
+      for (int j = i + 1; j < (int)ELL_W; ++j) {
+        const bool j_first = A1[j] < A1[i] || (A1[j] == A1[i] && TV[j] < TV[i]);
+        rank[i] += j_first ? 1 : 0;
+        rank[j] += j_first ? 0 : 1;
+      }
+    // the accept loop of replay()
+    float cur = INF;
+    EvFull tc = full_normal(cur, c);
+    win = -1;
+#pragma unroll
+    for (int r = 0; r < (int)ELL_W; ++r) {
+      if (r >= n) break;
+      float a1 = 0.0f, u1 = 0.0f, u2 = 0.0f; uint32_t Tv = 0u; int k = 0;
+#pragma unroll
+      for (int j = 0; j < (int)ELL_W; ++j)
+        if (rank[j] == r) { a1 = A1[j]; Tv = TV[j]; u1 = U1[j]; u2 = U2[j]; k = j; }
+      const EvTime T = ev_normal(a1, Tv);
+      if (!less_T_full(T, tc)) break;   // c has been popped before this face fires
+      const float4 wr = __ldg(&wrow[k]);
+      CvpResult res;
+      if (cvp_update_t<false>(u1, u2, cur, wr.z, wr.y, wr.x, res) && backstep_ok(res.value, T, Tv, round)) {
+        cur = res.value; accept(c, res.value, T, tc); win = k; ww = wr; wu1 = u1; wu2 = u2;
+      }
+    }
+    return true;
+  }
+
+  // the epilogue of c through replay() on the CSR records, out of line with its own frame (replay_row's other cases)
+  __device__ __noinline__ void epilogue_csr(uint32_t c, float goal) {
+    int win; float nd, wu1 = 0.0f, wu2 = 0.0f; EvFull nt;
+    replay(c, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, nd, nt, win, wu1, wu2);
+    write_aux(c, win, wu1, wu2);
   }
 
   // engine hook: returns true if the label changed (and stores it)
