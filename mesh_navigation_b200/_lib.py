@@ -122,5 +122,10 @@ def load():
     L.mnb_cancel.restype = i32; L.mnb_cancel.argtypes = [vp]
     L.mnb_get_stats.restype = i32; L.mnb_get_stats.argtypes = [vp, C.POINTER(Stats)]
     L.mnb_set_tuning.restype = i32; L.mnb_set_tuning.argtypes = [vp, f32, i32, i32]
+    # test hooks outside the header (meshnav.cu): the single-plan CVP epilogue's replay path, its hand-off count, the labels
+    L.mnb_debug_set_cvp_epilogue.restype = i32; L.mnb_debug_set_cvp_epilogue.argtypes = [vp, i32]
+    L.mnb_debug_get_epilogue_csr.restype = i32; L.mnb_debug_get_epilogue_csr.argtypes = [vp, C.POINTER(C.c_uint32)]
+    L.mnb_debug_get_labels.restype = i32; L.mnb_debug_get_labels.argtypes = [vp, vp]
+    L.mnb_debug_get_label_sides.restype = i32; L.mnb_debug_get_label_sides.argtypes = [vp, vp, vp, vp, u32]
     _lib = L
     return L

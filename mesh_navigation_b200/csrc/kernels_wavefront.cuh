@@ -237,13 +237,14 @@ __device__ __forceinline__ void cvp_epilogue_problem(const CvpKernelArgs& a, uin
 // row in registers (CvpProblem::replay_row), and a vertex it does not cover (more than 8 faces, a cascade member among the
 // sources) is handed to csr(c), which runs CvpProblem::epilogue_csr -- at once or in a launch of its own.  !ROW: the CSR
 // replay in line, for a caller whose registers cannot hold a row: at the 64 registers of the batch kernels the row
-// replay spills, and the batch with fields was measured 13 % slower with it.
-template <bool ROW, class Csr>
+// replay spills, and the batch with fields was measured 13 % slower with it.  ALL_CSR (with ROW; a test hook): every vertex
+// the row replay would take is handed to csr(c) instead, so that the two replays can be compared on the same labels.
+template <bool ROW, bool ALL_CSR = false, class Csr>
 __device__ __forceinline__ void cvp_epilogue_vertex(CvpProblem& prob, const int4* __restrict__ ell_idx, const float4* __restrict__ ell_w,
                                                     GroupCtl* ctl, uint32_t sf, float goal, uint32_t c, Csr csr) {
   const int4* row = ell_idx + (size_t)c * ELL_W;
   int4 ix[ELL_W];                                        // (requested together with the label of c)
-  if constexpr (ROW) {
+  if constexpr (ROW && !ALL_CSR) {
 #pragma unroll
     for (int j = 0; j < (int)ELL_W; ++j) ix[j] = __ldg(&row[j]);
   }
@@ -265,7 +266,7 @@ __device__ __forceinline__ void cvp_epilogue_vertex(CvpProblem& prob, const int4
   } else {
     if (__float_as_uint(d) == INF_BITS || !prob.eligible(c)) { prob.write_aux_none(c); return; }
     int win; float4 ww; float wu1, wu2;
-    if (!prob.replay_row(c, ix, ell_w, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, win, ww, wu1, wu2)) {
+    if (ALL_CSR || !prob.replay_row(c, ix, ell_w, __uint_as_float(INF_BITS), goal, 0xfffffff0u /* final labels: nothing is deferred */, win, ww, wu1, wu2)) {
       csr(c);
       return;
     }
@@ -394,10 +395,12 @@ __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpK
 // launches: k_cvp_epilogue replays every vertex its ELL row covers, in registers, and lists the others (ws.list1, free once
 // the wave has ended; ctl->epi_csr entries, cleared by the host before the launch); k_cvp_epilogue_csr replays those on
 // their CSR records.  A call to the out-of-line replay would cost the first kernel its registers: the call convention
-// caps them and saves the live ones to a stack frame.
+// caps them and saves the live ones to a stack frame.  ALL_CSR (mnb_debug_set_cvp_epilogue(ctx, 1), tests only): every
+// vertex the row replay covers is listed as well, so that the second launch replays them all on their CSR records.
 #ifndef MNB_EPILOGUE_THREADS
 #define MNB_EPILOGUE_THREADS 256
 #endif
+template <bool ALL_CSR = false>
 __global__ void __launch_bounds__(MNB_EPILOGUE_THREADS) k_cvp_epilogue(const CvpKernelArgs a, GroupCtl* ctl) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= a.V) return;
@@ -405,7 +408,7 @@ __global__ void __launch_bounds__(MNB_EPILOGUE_THREADS) k_cvp_epilogue(const Cvp
   CvpProblem prob;
   cvp_epilogue_problem(a, a.ws.state, a.ws.ext, a.ws.root, a.ws.chg, a.ws.pool, ctl, sf, a.seed_pos, time_get(ctl->goal_time),
                        a.out_pred, a.out_dir, a.out_cut, prob);
-  cvp_epilogue_vertex<true>(prob, a.ell_idx, a.ell_w, ctl, sf, __uint_as_float(ctl->goal_bits), c,
+  cvp_epilogue_vertex<true, ALL_CSR>(prob, a.ell_idx, a.ell_w, ctl, sf, __uint_as_float(ctl->goal_bits), c,
                       [&](uint32_t v) { a.ws.list1[atomicAdd(&ctl->epi_csr, 1u)] = v; });
 }
 __global__ void __launch_bounds__(256) k_cvp_epilogue_csr(const CvpKernelArgs a, GroupCtl* ctl) {

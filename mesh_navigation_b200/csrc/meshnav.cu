@@ -123,6 +123,7 @@ struct MeshState : RayCasterState {
   // mnb_cvp_replan: the resident wave of the last successful replan in its own workspace (labels, side arrays, level pool,
   // marks, lists, sweep versions, control block; allocated by the first replan) and what it was computed for
   WaveBuffers rw;
+  bool epi_in_rw = false;        // the last single plan's epilogue ran on rw (mnb_debug_get_epilogue_csr), not on ws
   bool rw_valid = false; uint32_t rw_seed_face = 0, rw_seed_pos[3] = {0, 0, 0}; uint64_t rw_cost_limit = 0, rw_cost_gen = 0;
   uint32_t rw_pool_top = 0;
   DeviceBuffer<uint32_t> d_replan_chg, d_replan_t0;      // the changed list of a replan, T0 and the block minima of its reduction
@@ -171,6 +172,7 @@ struct mnb_ctx : MeshState {
   bool layers_explicit = false;
   uint32_t replan_pool_room = 0;   // level-pool words a resumed replan wave may add (mnb_debug_set_replan_pool_room; 0 = the pool's)
   int sweeps = -1;             // in-round sweeps of the whole-grid single plans (mnb_debug_set_sweeps); -1 = derived from the band width
+  int cvp_epilogue = 0;        // single-plan epilogue (mnb_debug_set_cvp_epilogue): 0 row replay where it applies, 1 CSR replay for all
   float grid_delta = 1.8f;     // band width of the whole-grid single-plan kernel (wide band + in-round sweeps)
   float dijkstra_grid_delta = 3.0f;
   float dijkstra_batch_delta = 0.18f;
@@ -889,7 +891,10 @@ static int32_t launch_single_cvp(mnb_ctx* ctx, CvpKernelArgs a) {
     if (e != cudaSuccess) { ctx->err = std::string("cvp launch: ") + cudaGetErrorString(e); return MNB_E_CUDA; }
   }
   CK(cudaMemsetAsync(&a.ws.ctl->epi_csr, 0, sizeof(unsigned int), ctx->stream));
-  MNB_LAUNCH(k_cvp_epilogue, (ctx->V + MNB_EPILOGUE_THREADS - 1) / MNB_EPILOGUE_THREADS, MNB_EPILOGUE_THREADS, 0, ctx->stream, a, a.ws.ctl);
+  const unsigned epi_blocks = (ctx->V + MNB_EPILOGUE_THREADS - 1) / MNB_EPILOGUE_THREADS;
+  if (ctx->cvp_epilogue == 1) MNB_LAUNCH(k_cvp_epilogue<true>, epi_blocks, MNB_EPILOGUE_THREADS, 0, ctx->stream, a, a.ws.ctl);
+  else MNB_LAUNCH(k_cvp_epilogue<false>, epi_blocks, MNB_EPILOGUE_THREADS, 0, ctx->stream, a, a.ws.ctl);
+  ctx->epi_in_rw = a.ws.ctl == ctx->rw.ctl.p;
   MNB_LAUNCH(k_cvp_epilogue_csr, (unsigned)(4 * ctx->sm_count), 256, 0, ctx->stream, a, a.ws.ctl);   // (grid-stride over the list)
   CK(cudaGetLastError());
   return MNB_OK;
@@ -1395,6 +1400,20 @@ int32_t mnb_debug_set_replan_pool_room(mnb_ctx* ctx, uint32_t words) { if (!ctx)
 
 int32_t mnb_debug_set_infl_skip(mnb_ctx* ctx, int32_t on) { if (!ctx) return MNB_E_ARG; ctx->infl_skip_clean = on != 0; return MNB_OK; }
 int32_t mnb_debug_set_layers_smem(mnb_ctx* ctx, int32_t mode) { if (!ctx || mode < 0 || mode > 9) return MNB_E_ARG; ctx->layers_smem = mode; ctx->layers_explicit = true; return MNB_OK; }
+
+// test hooks (not part of the public header) of the single-plan CVP epilogue.  set: 0 (default) replays a vertex on its
+// ELL row where that covers it and hands the others to the CSR replay; 1 hands every vertex that is replayed at all (reached,
+// eligible, not a seed) to the CSR replay, so that tests can compare the two on the same labels.  get: the number of
+// vertices the last single plan's epilogue handed to the CSR replay (ctl->epi_csr of the workspace it ran on: the
+// resident one for mnb_cvp_replan)
+int32_t mnb_debug_set_cvp_epilogue(mnb_ctx* ctx, int32_t mode) { if (!ctx || mode < 0 || mode > 1) return MNB_E_ARG; ctx->cvp_epilogue = mode; return MNB_OK; }
+int32_t mnb_debug_get_epilogue_csr(mnb_ctx* ctx, uint32_t* n) {
+  if (!ctx || !n) return MNB_E_ARG;
+  const GroupCtl* ctl = ctx->epi_in_rw ? ctx->rw.ctl.p : ctx->ws.ctl.p;
+  if (!ctl) return MNB_E_STATE;
+  CK(cudaMemcpy(n, &ctl->epi_csr, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  return MNB_OK;
+}
 
 // debugging aid (not part of the public header): raw labels {d, a1, a2, a3|flag} of wavefront group 0
 int32_t mnb_debug_get_labels(mnb_ctx* ctx, uint32_t* out4v) {

@@ -1,7 +1,8 @@
 """Batched CVP vector fields (mnb_cvp_batch_fields / CVPMeshPlanner.waveFrontPropagationBatchFields): every row of the
 potential, predecessor, direction and cutting-face outputs against mnb_cvp with the same goal (robot face -1) bit for bit,
 and against the oracle's CVPMeshPlanner::waveFrontPropagation (cvp_mesh_planner.cpp:651-886) -- potentials bit for bit,
-predecessors and cutting faces exactly, directions within 1e-5.  The GPU tests run with -m gpu on an H100; the last test
+predecessors and cutting faces exactly, directions bit for bit on the CPU interpreter and on the GPU at most one float ulp
+apart on fewer than 1e-4 of the vertices (CUDA's and glibc's double acos may differ in the last bit).  The GPU tests run with -m gpu on an H100; the last test
 replays them on the CPU interpreter of the kernels (tests/emu)."""
 import ctypes as C
 import os
@@ -51,6 +52,17 @@ def _same(a, b):
     return a.shape == b.shape and (a.view(np.uint32) == b.view(np.uint32)).all()
 
 
+def _direction_ok(got, ref):
+    """directions against the oracle's: bit for bit on the CPU interpreter (its acos is the oracle's); on the GPU at most
+    one float ulp apart, on fewer than 1e-4 of the vertices"""
+    from mesh_navigation_b200 import _lib
+    line = lambda x: (lambda i: np.where(i < 0, -(i & 0x7FFFFFFF), i))(np.asarray(x, np.float32).view(np.int32).astype(np.int64))
+    u = np.abs(line(got) - line(ref))
+    if _lib.LIB_PATH.endswith("libmeshnav_emu.so"):
+        return (u == 0).all()
+    return u.max() <= 1 and np.count_nonzero(u) < 1e-4 * u.size
+
+
 def _check_oracle(om, w, vc, sfs, sps, got, invalid=None, cost_limit=1.0, rows=None):
     for k in (range(len(sfs)) if rows is None else rows):
         ref = om.cvp(w, vc, int(sfs[k]), sps[k], invalid=invalid, cost_limit=cost_limit)
@@ -61,7 +73,7 @@ def _check_oracle(om, w, vc, sfs, sps, got, invalid=None, cost_limit=1.0, rows=N
         if got["cutting_face"] is not None:
             assert (got["cutting_face"][k] == ref["cutting_face"]).all(), f"row {k}: cutting_face"
         if got["direction"] is not None:
-            assert np.abs(got["direction"][k] - ref["direction"]).max() <= 1e-5, f"row {k}: direction"
+            assert _direction_ok(got["direction"][k], ref["direction"]), f"row {k}: direction"
 
 
 def _check_single(pl, sfs, sps, got, rows=None):
@@ -139,7 +151,7 @@ def test_cvp_batch_fields_hard_cases(api, oracle_mod, name):
                 assert _same(got[key][k], singles[k][key]), (cluster, delta, k, key)
             assert _same(got["dist"][k], refs[k]["dist"]), (cluster, delta, k)
             assert (got["pred"][k] == refs[k]["pred"]).all() and (got["cutting_face"][k] == refs[k]["cutting_face"]).all(), (cluster, delta, k)
-            assert np.abs(got["direction"][k] - refs[k]["direction"]).max() <= 1e-5, (cluster, delta, k)
+            assert _direction_ok(got["direction"][k], refs[k]["direction"]), (cluster, delta, k)
         if name.startswith("deep_cascade"):
             assert got["deep_labels"] >= singles[0]["deep_labels"] > 0          # counted by the per-wave epilogue
     mm.close()
@@ -216,7 +228,7 @@ def test_cvp_batch_fields_counts(api, oracle_mod):
             ref[int(f)] = om.cvp(w, vc, int(f), sps[k])
         r = ref[int(f)]
         assert _same(got["dist"][k], r["dist"]) and (got["pred"][k] == r["pred"]).all(), k
-        assert (got["cutting_face"][k] == r["cutting_face"]).all() and np.abs(got["direction"][k] - r["direction"]).max() <= 1e-5, k
+        assert (got["cutting_face"][k] == r["cutting_face"]).all() and _direction_ok(got["direction"][k], r["direction"]), k
     mm.close()
 
 

@@ -45,7 +45,7 @@ for case in range(N):
     ref = om.cvp(w, vc, sf, sp, rf, invalid=inv, cost_limit=cl)
     got = api.CVPMeshPlanner(mm, cost_limit=cl).waveFrontPropagation(sf, sp, rf)
     if got["outcome"] != ref["outcome"] or (got["dist"].view(np.uint32) != ref["dist"].view(np.uint32)).any() or (got["pred"] != ref["pred"]).any() \
-            or (got["cutting_face"] != ref["cutting_face"]).any():
+            or (got["cutting_face"] != ref["cutting_face"]).any() or (got["direction"].view(np.uint32) != ref["direction"].view(np.uint32)).any():
         msg.append(f"CVP outcome {got['outcome']}/{ref['outcome']} dist!= {(got['dist'].view(np.uint32) != ref['dist'].view(np.uint32)).sum()} pred!= {(got['pred'] != ref['pred']).sum()} "
                    f"cut!= {(got['cutting_face'] != ref['cutting_face']).sum()} at {np.where(got['cutting_face'] != ref['cutting_face'])[0][:4].tolist()}")
     # the lean batch round loop (k_cvp_batch): three goals, random cluster size / band width
