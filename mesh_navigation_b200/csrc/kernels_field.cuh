@@ -355,6 +355,7 @@ struct BacktrackArgs {
   double step_width; uint32_t max_points;
   float* path_pos; uint32_t* path_face; int32_t* result /* [0] outcome, [1] n_points */; const int* cancel_flag;
   RepulsiveField layer;        // InflationLayer::vectorAt added in meshAhead (mesh_map.cpp:1097-1102); dist == null: none
+  uint32_t* spill_list; uint32_t* spill_key;   // F entries each, keys all zero (bt_search_spill); null: not reserved yet
 };
 
 __device__ __forceinline__ bool projected_barycentric(F3 p, F3 a, F3 b, F3 c, float bary[3], float& dist) {
@@ -375,7 +376,83 @@ __device__ __forceinline__ bool projected_barycentric(F3 p, F3 a, F3 b, F3 c, fl
 // the lanes 32 faces at a time: containment tests in parallel, expansions gathered per lane, deduplicated through a
 // shared-memory hash set and appended in exactly the order the sequential loop of mesh_map.cpp:1031-1063 would
 // produce (lane-major sequence numbers + atomicMin decide which duplicate came first), so the face that is returned
-// is the same one.
+// is the same one.  A search that outgrows the shared-memory list (fine meshes: ~5000 faces per 0.4 m step at 1 cm)
+// or a candidate row (a listed face next to a vertex of high degree) runs again from its start in bt_search_spill,
+// which has no limit below F faces; a walk that needs it before the host reserved its workspace ends with
+// BT_NEEDS_SPILL, and the host reserves it and walks again.
+constexpr int32_t BT_NEEDS_SPILL = -100;   // internal outcome, never returned by the C ABI
+constexpr uint32_t BT_MEMBER = 0xffffffffu;
+
+// searchNeighbourFaces in global memory: the list in spill_list; spill_key[f] is 0 for a face not seen, BT_MEMBER for
+// a listed one and, while one round of 32 listed faces is expanded, the largest key (= the first in the sequential
+// order) of the candidates that name it.  Every face a round touches is listed when the round ends, so clearing the
+// keys of the listed faces leaves the array all zero for the next search.  Keys are read with __ldcg: the atomics
+// write them in L2.
+__device__ bool bt_search_spill(const BacktrackArgs& a, F3 pos, F3 center, float rsq, uint32_t& face, float bary[3]) {
+  constexpr unsigned FULL = 0xffffffffu;
+  const uint32_t lane = threadIdx.x;
+  uint32_t* const list = a.spill_list; uint32_t* const key = a.spill_key;
+  if (lane == 0) { list[0] = face; key[face] = BT_MEMBER; }
+  __syncwarp();
+  uint32_t cnt = 1, it = 0;
+  bool ok = false;
+  while (it < cnt) {
+    const uint32_t chunk = min(32u, cnt - it);
+    const bool act = lane < chunk;
+    const uint32_t f = act ? __ldcg(list + it + lane) : 0u;
+    const uint32_t* q = a.faces + 3 * (size_t)f;
+    const uint32_t qv[3] = {q[0], q[1], q[2]};
+    const F3 PV[3] = {f3load(a.pos, qv[0]), f3load(a.pos, qv[1]), f3load(a.pos, qv[2])};
+    float lb[3], ld;
+    const bool pass = act && projected_barycentric(pos, PV[0], PV[1], PV[2], lb, ld) && fabsf(ld) < 0.4f;
+    const unsigned pm = __ballot_sync(FULL, pass);
+    if (pm) {
+      const int L = __ffs(pm) - 1;
+      face = __shfl_sync(FULL, f, L);
+      bary[0] = __shfl_sync(FULL, lb[0], L); bary[1] = __shfl_sync(FULL, lb[1], L); bary[2] = __shfl_sync(FULL, lb[2], L);
+      ok = true;
+      break;
+    }
+    // my candidates: the corner rows of my vertices within the radius, in the reference's order
+    uint32_t lo[3], hi[3], nc = 0;
+    for (int k = 0; k < 3; ++k) {
+      lo[k] = hi[k] = 0;
+      const F3 e = f3sub(center, PV[k]);
+      if (act && f3dot(e, e) < rsq) { lo[k] = a.cor_ptr[qv[k]]; hi[k] = a.cor_ptr[qv[k] + 1]; }
+      nc += hi[k] - lo[k];
+    }
+    uint32_t base = nc;                                  // lane-major sequence number of my first candidate
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, base, o); if ((int)lane >= o) base += v; }
+    base -= nc;
+    auto key_of = [](uint32_t seq) { return BT_MEMBER - 1u - seq; };   // earlier in the sequential order: larger
+    uint32_t s = base;
+    for (int k = 0; k < 3; ++k)
+      for (uint32_t j = lo[k]; j < hi[k]; ++j) atomicMax(&key[(uint32_t)a.cor_idx[j].z], key_of(s++));
+    __syncwarp();
+    uint32_t newc = 0;                                   // candidates whose key survived: the first of their face
+    s = base;
+    for (int k = 0; k < 3; ++k)
+      for (uint32_t j = lo[k]; j < hi[k]; ++j) newc += __ldcg(&key[(uint32_t)a.cor_idx[j].z]) == key_of(s++) ? 1u : 0u;
+    uint32_t incl = newc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if ((int)lane >= o) incl += v; }
+    const uint32_t total = __shfl_sync(FULL, incl, 31);
+    uint32_t w = cnt + incl - newc;
+    s = base;                                            // append them in order; listed faces are members from now on
+    for (int k = 0; k < 3; ++k)
+      for (uint32_t j = lo[k]; j < hi[k]; ++j) {
+        const uint32_t c = (uint32_t)a.cor_idx[j].z;
+        if (__ldcg(&key[c]) == key_of(s++)) { list[w++] = c; key[c] = BT_MEMBER; }
+      }
+    __syncwarp();
+    cnt += total; it += chunk;
+  }
+  for (uint32_t j = lane; j < cnt; j += 32) key[__ldcg(list + j)] = 0u;
+  __syncwarp();
+  return ok;
+}
+
 constexpr int BT_LIST_CAP = 4096;      // faces in the search list
 constexpr int BT_HASH_CAP = 8192;      // open-addressing set over face ids (power of two)
 constexpr int BT_MAXC = 64;            // expansion candidates of one listed face (<= sum of its vertices' face counts)
@@ -497,7 +574,11 @@ __global__ void __launch_bounds__(32) k_backtrack(BacktrackArgs a) {
         __syncwarp();
         cnt += total; it += chunk;
       }
-      if (!ok) { outcome = overflow ? MNB_E_STATE : MNB_NO_PATH_FOUND; break; }
+      if (overflow) {
+        if (!a.spill_list) { outcome = BT_NEEDS_SPILL; break; }
+        ok = bt_search_spill(a, pos, center, rsq, face, bary);
+      }
+      if (!ok) { outcome = MNB_NO_PATH_FOUND; break; }
       t = a.faces + 3 * (size_t)face;
       const F3 A = f3load(a.pos, t[0]), B = f3load(a.pos, t[1]), C = f3load(a.pos, t[2]);   // project onto the surface
       pos = {A.x * bary[0] + B.x * bary[1] + C.x * bary[2], A.y * bary[0] + B.y * bary[1] + C.y * bary[2],

@@ -128,6 +128,7 @@ struct MeshState : RayCasterState {
   uint32_t rw_pool_top = 0;
   DeviceBuffer<uint32_t> d_replan_chg, d_replan_t0;      // the changed list of a replan, T0 and the block minima of its reduction
   DeviceBuffer<float> d_path_pos; DeviceBuffer<uint32_t> d_path_face; DeviceBuffer<int32_t> d_bt_result;
+  DeviceBuffer<uint32_t> d_bt_spill_list, d_bt_spill_key;   // F each: k_backtrack's unbounded face search (first walk that needs it)
   DeviceBuffer<uint8_t> d_infl_invalid;
   // repulsive vector field of the last inflation (InflationLayer::vector_map_ / distances_)
   bool infl_labels_valid = false, infl_had_invalid = false, infl_field_valid = false, repulsive_on = false;
@@ -1346,20 +1347,28 @@ static int32_t impl_cvp_backtrack(mnb_ctx* ctx, const float robot_pos[3], uint32
   a.path_pos = io.out(path_pos, ctx->d_path_pos.p, 3, &n); a.path_face = io.needed(path_face, ctx->d_path_face.p, 1, &n); a.result = ctx->d_bt_result; a.cancel_flag = ctx->d_cancel;
   a.layer = RepulsiveField{};
   if (ctx->repulsive_on && ctx->infl_field_valid) a.layer = repulsive_field_of(ctx);
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
   CK(cudaFuncSetAttribute(k_backtrack, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BtShared)));
-  MNB_LAUNCH(k_backtrack, 1, 32, sizeof(BtShared), ctx->stream, a);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(ctx->ev1, ctx->stream));
   int32_t res[2] = {0, 0};
-  CK(cudaMemcpyAsync(res, ctx->d_bt_result, sizeof(res), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+  for (;;) {
+    a.spill_list = ctx->d_bt_spill_list; a.spill_key = ctx->d_bt_spill_key;
+    CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    MNB_LAUNCH(k_backtrack, 1, 32, sizeof(BtShared), ctx->stream, a);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->ev1, ctx->stream));
+    CK(cudaMemcpyAsync(res, ctx->d_bt_result, sizeof(res), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (res[0] != BT_NEEDS_SPILL) break;
+    // a face search outgrew shared memory: reserve the unbounded one (keys all zero) and walk again -- the walk is
+    // deterministic, so the second one returns what one walk with the workspace would
+    CK(ctx->d_bt_spill_list.reserve(ctx->F)); CK(ctx->d_bt_spill_key.reserve(ctx->F));
+    CK(cudaMemsetAsync(ctx->d_bt_spill_key, 0, sizeof(uint32_t) * (size_t)ctx->F, ctx->stream));
+  }
   n = (uint32_t)res[1] < max_points ? (uint32_t)res[1] : max_points;
   *n_points = n;
   CK(io.copy_back());
   CK(cudaStreamSynchronize(ctx->stream));
   simple_stats(ctx, 1, n);
-  if (res[0] == MNB_E_STATE) { ctx->err = "back-tracking exceeded max_points (cyclic vector field?) or the face search list"; return MNB_E_STATE; }
+  if (res[0] == MNB_E_STATE) { ctx->err = "back-tracking exceeded max_points (cyclic vector field?)"; return MNB_E_STATE; }
   return res[0];
 }
 

@@ -298,7 +298,12 @@ def _cvp_vector_map(self, vertex_normals, pred, direction, cutting_face):
 def _cvp_backtrack(self, vector_map, start, start_face, goal, goal_face, step_width=0.4, max_points=100000, repulsive=None):
     """cvp:920-951: walk from `goal` (robot) down the field to `start` (wave seed); returns (outcome, positions, faces).
     repulsive: optional dict(dist, vectors, inscribed_radius, inflation_radius, lethal_value, inscribed_value) -- the
-    InflationLayer field meshAhead adds (mesh_map.cpp:1097-1102, inflation_layer.cpp:493-521)"""
+    InflationLayer field meshAhead adds (mesh_map.cpp:1097-1102, inflation_layer.cpp:493-521).
+    A face outside [0, F) returns no points: INVALID_START (52) for `start_face`, INVALID_GOAL (53) for `goal_face`, as
+    mnb_cvp / mnb_cvp_backtrack do."""
+    for code, f in ((52, start_face), (53, goal_face)):
+        if not 0 <= int(f) < self.F:
+            return code, np.empty((0, 3), np.float32), np.empty(0, np.uint32)
     vm = np.ascontiguousarray(vector_map, dtype=np.float32)
     st = np.ascontiguousarray(start, dtype=np.float32); go = np.ascontiguousarray(goal, dtype=np.float32)
     pp = np.empty((max_points, 3), np.float32); pf = np.empty(max_points, np.uint32); n = C.c_uint32(0)
