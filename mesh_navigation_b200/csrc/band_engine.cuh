@@ -291,9 +291,10 @@ struct GroupCtl {               // one per wavefront group, global memory
   unsigned int count[3];        // candidate list sizes (ring over rounds)
   unsigned int m_tau[3];        // float bits: min tau touched by a change in the round
   unsigned int lo[3];           // float bits: min pop time over surviving candidates
-  // goal_dist (cvp:738,769 / dijkstra:279,296) and the cancel flag are read by EVERY thread at the
-  // top of a round and decide whether the group leaves the loop, so they must not change while a
-  // round is running: round r reads slot r&1, writers of round r only touch slot (r+1)&1.
+  // goal_dist (cvp:738,769 / dijkstra:279,296), the stop / cancel flag and (matrix form) done_ring are read by EVERY
+  // thread at the top of a round and decide whether the group leaves the loop, so they must not change while a round is
+  // running: round r reads slot r&1, writers of round r only touch slot (r+1)&1 (band_advance).  So every exit is
+  // group-uniform and the group barrier at the end of a round cannot hang.
   unsigned int goal_ring[2];    // float bits, monotonically decreasing (atomicMin)
   unsigned int stop_ring[2];
   unsigned int goal_bits;       // final goal_dist, published after the last round
@@ -315,8 +316,9 @@ struct GroupCtl {               // one per wavefront group, global memory
   unsigned int barrier[2];      // grid_barrier state (whole-grid groups only)
   unsigned long long t_ph[8];   // phase cycles of thread 0 inside one candidate iteration (debug)
   // matrix form of the batch kernels (TargetSet): distinct targets of the wave that have not settled yet, and the flag
-  // that ends the wave once none is left.  The flag is read at the top of a round like stop_ring, so it follows the same
-  // discipline: round r reads slot r&1, the thread that settles the last target in round r raises slot (r+1)&1.
+  // that ends the wave once none is left (raised by the thread that settles the last target).  It needs no carrying or
+  // clearing: the loop ends at the first round that reads it raised, so slot (r+1)&1 was read clear in round r-1 and
+  // nobody has written it since.
   int targets_left;
   unsigned int done_ring[2];
   unsigned int epi_csr;         // k_cvp_epilogue: vertices it listed for the CSR replay of k_cvp_epilogue_csr
@@ -440,6 +442,14 @@ __device__ __forceinline__ void stage_flush(S& st, uint32_t* list_next, unsigned
   // before the next round's pushes
 }
 
+// k consecutive slots of the counter *cnt for the whole warp, with one atomic (every lane of the warp calls this and gets
+// the first slot)
+__device__ __forceinline__ unsigned int warp_reserve(unsigned int* cnt, const unsigned int k) {
+  unsigned int base = 0u;
+  if ((threadIdx.x & 31) == 0) base = atomicAdd(cnt, k);
+  return __shfl_sync(0xffffffffu, base, 0);
+}
+
 // A vertex c with label `old` settles in round r: if it is the last of the robot face's vertices r0-r2 to settle, the goal
 // cutoff is armed at the latest pop time of the three (c is not necessarily the last of them in event order), and the
 // goal distance follows from that vertex's potential.
@@ -460,19 +470,43 @@ __device__ __forceinline__ void arm_goal_cutoff(const P& prob, GroupCtl* ctl, co
   }
 }
 
-// the end of a wave after r rounds: the thread's counters, and (thread 0 of the group) the round count, the strict rule,
-// the watchdog and the final goal distance
+// Thread 0 of the group prepares round r + 1 of a round loop (r % 3 = this round's slot): it clears list r+2's counter (free
+// during this round) and the minima of round r+1, carries the goal cutoff (GOAL) and writes the stop flag of round r+1
+// from this round's, the cancel flag (polled every 32 rounds) and (STOP_ON_OVERFLOW) the level pool's overflow flag.
+template <bool GOAL, bool STOP_ON_OVERFLOW = false>
+__device__ __forceinline__ void band_advance(GroupCtl* ctl, const uint32_t gtid, const uint32_t r, const unsigned int goal_b, const unsigned int stop,
+                                             const volatile int* cancel_flag) {
+  if (gtid == 0) {
+    ctl->count[(r + 2) % 3] = 0;
+    ctl->m_tau[(r + 1) % 3] = INF_BITS;
+    ctl->lo[(r + 1) % 3] = INF_BITS;
+    if constexpr (GOAL) atomicMin(&ctl->goal_ring[(r + 1) & 1], goal_b);
+    if constexpr (STOP_ON_OVERFLOW)
+      ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag) || __ldcg(&ctl->pool_overflow)) ? 1u : 0u;
+    else
+      ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag)) ? 1u : 0u;
+  }
+}
+
+// thread 0 of the group at the end of a wave after r rounds: the round count, the strict rule, the watchdog and (GOAL) the
+// final goal distance
+template <bool GOAL>
+__device__ __forceinline__ void band_wave_end(GroupCtl* ctl, const uint32_t gtid, const uint32_t r, const uint32_t max_rounds, const int strict) {
+  if (gtid == 0) {
+    ctl->rounds += r;
+    if (strict) ctl->strict_armed += 1;
+    if (r > max_rounds) ctl->watchdog = 1;
+    if constexpr (GOAL) ctl->goal_bits = min(ctl->goal_ring[0], ctl->goal_ring[1]);
+  }
+}
+
+// the end of a wave after r rounds: the thread's counters, then band_wave_end
 __device__ __forceinline__ void band_stats(GroupCtl* ctl, const uint32_t gtid, const uint32_t r, const uint32_t max_rounds, const int strict,
                                            const unsigned long long recomputes, const unsigned long long settled, const unsigned long long skipped) {
   atomicAdd(&ctl->recomputes, recomputes);
   atomicAdd(&ctl->settled, settled);
   if (skipped) atomicAdd(&ctl->skipped, skipped);
-  if (gtid == 0) {
-    ctl->rounds += r;
-    if (strict) ctl->strict_armed += 1;
-    if (r > max_rounds) ctl->watchdog = 1;
-    ctl->goal_bits = min(ctl->goal_ring[0], ctl->goal_ring[1]);
-  }
+  band_wave_end<true>(ctl, gtid, r, max_rounds, strict);
 }
 
 // -----------------------------------------------------------------------------
@@ -513,26 +547,18 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
     if constexpr (P::HAS_GOAL_TIME) if (has_robot && goal_b != INF_BITS) prob.goal_t = time_get(ctl->goal_time);
     const unsigned int stop = __ldcg(&ctl->stop_ring[r & 1]);
     if (n == 0 || stop || r > max_rounds) break;  // r is group-uniform: the watchdog cannot deadlock the barrier
-    // every target has settled.  The flag needs no carrying or clearing: the loop ends at the first round that reads it
-    // raised, so slot (r+1)&1 was read clear in round r-1 and nobody has written it since.
-    if constexpr (TARGETS) if (__ldcg(&ctl->done_ring[r & 1])) break;
+    if constexpr (TARGETS) if (__ldcg(&ctl->done_ring[r & 1])) break;    // every target has settled
     if (r > 0 && __float_as_uint(m_prev) == INF_BITS &&
         (__float_as_uint(lo_prev) == INF_BITS || lo_prev > goal)) break;
     // stagnation watch (all values are group-uniform): labels keep changing but the earliest unsettled pop
     // time does not move -> a dependency cycle between a trigger and its back-step child; arm the strict rule
-    if (r > 0 && __float_as_uint(m_prev) != INF_BITS && !(lo_prev > lo_best)) { if (++stagnant >= P::STAGNATION) prob.strict = 1; }
+    if (r > 0 && __float_as_uint(m_prev) != INF_BITS && !(lo_prev > lo_best)) { if (++stagnant >= STAGNATION_ROUNDS) prob.strict = 1; }
     else { stagnant = 0; if (lo_prev > lo_best) lo_best = lo_prev; }
     float band_end = lo_prev + delta;
     if (!(band_end > band_end_prev)) band_end = band_end_prev;
     uint32_t* list_r = (r & 1) ? list1 : list0;
     uint32_t* list_n = (r & 1) ? list0 : list1;
-    if (gtid == 0) {
-      ctl->count[(r + 2) % 3] = 0;         // list r+2's counter (free during this round)
-      ctl->m_tau[next] = INF_BITS;
-      ctl->lo[next] = INF_BITS;
-      atomicMin(&ctl->goal_ring[(r + 1) & 1], goal_b);                 // carry the cutoff into the next round
-      ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag)) ? 1u : 0u;
-    }
+    band_advance<true>(ctl, gtid, r, goal_b, stop, cancel_flag);
 #ifdef MNB_EMU_ACTIVE   // round trace on the CPU interpreter of the kernels (tests/emu, MNB_EMU_TRACE=1): list length and progress per round
     if (gtid == 0 && getenv("MNB_EMU_TRACE")) fprintf(stderr, "[round %u] list %u m_prev %g lo_prev %g strict %d\n", r, n, m_prev, lo_prev, prob.strict);
 #endif
@@ -691,8 +717,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     if (!need_rescan && n == 0) break;
     if (!need_rescan && r > 0 && __float_as_uint(m_prev) == INF_BITS &&
         (__float_as_uint(lo_prev) == INF_BITS || lo_prev > goal)) break;
-    // stagnation watch (all values are group-uniform): labels keep changing but the earliest unsettled pop
-    // time does not move -> a dependency cycle between a trigger and its back-step child; arm the strict rule
+    // stagnation watch (see run_band_rounds)
     if (r > 0 && __float_as_uint(m_prev) != INF_BITS && !(lo_prev > lo_best)) { if (++stagnant >= STAGNATION_ROUNDS) prob.strict = 1; }
     else { stagnant = 0; if (lo_prev > lo_best) lo_best = lo_prev; }
     // the sweeps work on the first SW_CAP stage slots of a CTA: on very long fronts (tens of millions of vertices) the
@@ -709,14 +734,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     if (!(band_end > band_end_prev)) band_end = band_end_prev;
     uint32_t* list_r = (r & 1) ? list1 : list0;
     uint32_t* list_n = (r & 1) ? list0 : list1;
-    if (gtid == 0) {
-      ctl->count[(r + 2) % 3] = 0;
-      ctl->m_tau[next] = INF_BITS;
-      ctl->lo[next] = INF_BITS;
-      atomicMin(&ctl->goal_ring[(r + 1) & 1], goal_b);                 // carry the cutoff into the next round
-      ctl->stop_ring[(r + 1) & 1] = (stop || (cancel_flag && (r & 31) == 0 && *cancel_flag) ||
-                                     (STOP_ON_OVERFLOW && __ldcg(&ctl->pool_overflow))) ? 1u : 0u;
-    }
+    band_advance<true, STOP_ON_OVERFLOW>(ctl, gtid, r, goal_b, stop, cancel_flag);
     // Goal cutoff (cvp:754 / dijkstra:299) with a band wider than goal_dist_offset: labels computed before the cutoff
     // is known may rest on sources that turn out to lie beyond it.  Once it is known, (1) vertices beyond it never
     // settle any more -- they are recomputed under the cutoff until nothing changes -- and (2) the ones that had already
@@ -910,9 +928,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
           for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(FULL, incl, o); if (lane >= (unsigned)o) incl += y; }
           const unsigned int tot = __shfl_sync(FULL, incl, 31);
           if (tot) {
-            unsigned int base = 0u;
-            if (lane == 0) base = atomicAdd(&st.n, tot);
-            unsigned int p = __shfl_sync(FULL, base, 0) + incl - mine;
+            unsigned int p = warp_reserve(&st.n, tot) + incl - mine;
             if (done) stage_put_seen(st, *ss, p++, c, v0, nb, list_n, &ctl->count[next]);
             for (; won; won &= won - 1u) {
               const int b = __ffs(won) - 1;
@@ -923,9 +939,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
           const bool defer = has && !done;
           const unsigned dq = __ballot_sync(FULL, defer);
           if (dq) {
-            unsigned int qbase = 0u;
-            if (lane == 0) qbase = atomicAdd(&gq_n, (unsigned)__popc(dq));
-            qbase = __shfl_sync(FULL, qbase, 0);
+            const unsigned int qbase = warp_reserve(&gq_n, (unsigned)__popc(dq));
             if (defer) gq[qbase + __popc(dq & lt)] = c;
           }
         }

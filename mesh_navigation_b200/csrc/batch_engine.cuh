@@ -232,9 +232,7 @@ __device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup
         const unsigned b1 = __ballot_sync(FULL, p1), b2 = __ballot_sync(FULL, p2);
         const unsigned tot = (unsigned)(__popc(b1) + __popc(b2));
         if (tot) {
-          unsigned int base = 0;
-          if (lane == 0) base = atomicAdd(&st.n, tot);
-          base = __shfl_sync(FULL, base, 0);
+          const unsigned int base = warp_reserve(&st.n, tot);
           if (p1) batch_stage_write(st, base + __popc(b1 & lt), (uint32_t)ix.x, list_n, count_next);
           if (p2) batch_stage_write(st, base + __popc(b1) + __popc(b2 & lt), (uint32_t)ix.y, list_n, count_next);
         }
@@ -290,12 +288,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
     const uint32_t* list_r = (r & 1) ? list1 : list0;
     uint32_t* list_n = (r & 1) ? list0 : list1;
     unsigned int* const count_next = &ctl->count[next];
-    if (gtid == 0) {
-      ctl->count[(r + 2) % 3] = 0;
-      ctl->m_tau[next] = INF_BITS;
-      ctl->lo[next] = INF_BITS;
-      ctl->stop_ring[(r + 1) & 1] = (stop || (a.cancel_flag && (r & 31) == 0 && *(const volatile int*)a.cancel_flag)) ? 1u : 0u;
-    }
+    band_advance<false>(ctl, gtid, r, INF_BITS, stop, a.cancel_flag);
     const uint32_t buf_now = r & 1u, buf_prev = buf_now ^ 1u;      // re-labels of this round / of the previous round
     float my_mtau = INF, my_lo = INF;
     const unsigned int cnt = n > blk ? (n - blk + nblk - 1) / nblk : 0u;
@@ -324,15 +317,11 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
         if (keep) { my_skipped++; my_lo = fminf(my_lo, tau); }
         const unsigned km = __ballot_sync(FULL, keep), wm = __ballot_sync(FULL, work);
         if (km) {
-          unsigned int base = 0;
-          if (lane == 0) base = atomicAdd(&st.n, (unsigned)__popc(km));
-          base = __shfl_sync(FULL, base, 0);
+          const unsigned int base = warp_reserve(&st.n, (unsigned)__popc(km));
           if (keep) batch_stage_write(st, base + __popc(km & lt), ce, list_n, count_next);
         }
         if (wm) {
-          unsigned int base = 0;
-          if (lane == 0) base = atomicAdd(&wk.n, (unsigned)__popc(wm));
-          base = __shfl_sync(FULL, base, 0);
+          const unsigned int base = warp_reserve(&wk.n, (unsigned)__popc(wm));
           if (work) wk.q[base + __popc(wm & lt)] = ce;
         }
       }
@@ -372,10 +361,9 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
           if (changed || act_now) {
             // tell the face neighbours about the re-label (clean-candidate rule) / pull them into the candidate set (once)
             const uint32_t kb = __float_as_uint(fminf(tau, m));
-#ifndef MNB_BATCH_SERIAL_ACTIVATION
-            // The activation used to test mark[x] neighbour by neighbour inside the loop that also issues the CAS and the stage
-            // write: twelve dependent L2 round trips for the one evaluation per vertex that activates.  Now the marks of the whole ring are requested first (no store in
-            // that loop, so the loads overlap) and only the unmarked, eligible neighbours take the CAS.
+            // The marks of the whole ring are requested first (no store in that loop, so the loads overlap) and only the
+            // unmarked, eligible neighbours take the CAS: testing them one by one in the loop that issues the CAS and the stage
+            // write makes twelve dependent L2 round trips of the one evaluation per vertex that activates.
             uint32_t todo = 0u;
             if (act_now) {
 #pragma unroll
@@ -399,34 +387,15 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
                   batch_stage_write(st, atomicAdd(&st.n, 1u), x, list_n, count_next);
               }
             }
-#else
-            for (int k = 0; k < (int)ELL_W; ++k) {
-              const int4 ix = __ldg(&a.ell_idx[(size_t)c * ELL_W + k]);
-              if (ix.x == ELL_EMPTY) continue;
-              const uint32_t xs[2] = {(uint32_t)ix.x, (uint32_t)ix.y};
-#pragma unroll
-              for (int t = 0; t < 2; ++t) {
-                const uint32_t x = xs[t];
-                if (changed) atomicMin(&skw[4 * (size_t)x + buf_now], kb);
-                if (act_now && __ldcg(&G.mark[x]) == MARK_NONE && !(a.invalid && a.invalid[x]) && !((double)__ldg(&a.cost[x]) >= a.cost_limit) &&
-                    atomicCAS(&G.mark[x], MARK_NONE, MARK_CAND) == MARK_NONE)
-                  batch_stage_write(st, atomicAdd(&st.n, 1u), x, list_n, count_next);
-              }
-            }
-#endif
           }
         }
         const unsigned dm = __ballot_sync(FULL, done), fm = __ballot_sync(FULL, has && defer);
         if (dm) {   // the candidate survives into the next round's list (one shared atomic per warp)
-          unsigned int base = 0;
-          if (lane == 0) base = atomicAdd(&st.n, (unsigned)__popc(dm));
-          base = __shfl_sync(FULL, base, 0);
+          const unsigned int base = warp_reserve(&st.n, (unsigned)__popc(dm));
           if (done) batch_stage_write(st, base + __popc(dm & lt), c | (((ce & LIST_ACTIVATED) || act_now) ? LIST_ACTIVATED : 0u), list_n, count_next);
         }
         if (fm) {
-          unsigned int base = 0;
-          if (lane == 0) base = atomicAdd(&wk.ns, (unsigned)__popc(fm));
-          base = __shfl_sync(FULL, base, 0);
+          const unsigned int base = warp_reserve(&wk.ns, (unsigned)__popc(fm));
           if (has && defer) wk.sq[base + __popc(fm & lt)] = ce;
         }
       }
@@ -450,11 +419,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
     band_end_prev = band_end;
     group_sync<CS>();
   }
-  if (gtid == 0) {
-    ctl->rounds += r;
-    if (strict) ctl->strict_armed += 1;
-    if (r > a.max_rounds) ctl->watchdog = 1;
-  }
+  band_wave_end<false>(ctl, gtid, r, a.max_rounds, strict);
 #ifdef MNB_EMU_ACTIVE
   group_sync<CS>();
   if (gtid == 0 && getenv("MNB_EMU_TRACE")) fprintf(stderr, "[batch plan] rounds %u evaluations: still-inf %llu changed %llu unchanged %llu (general path %llu) settled %llu\n", r, ctl->t_ph[0], ctl->t_ph[1], ctl->t_ph[2], ctl->t_ph[3], ctl->settled);

@@ -24,7 +24,6 @@ namespace mnb {
 struct CvpProblem : LabelStore {
   static constexpr bool HAS_GOAL_TIME = true;
   EvTime goal_t;                            // pop time of the vertex that armed the goal cutoff (GroupCtl::goal_time); +inf: not armed
-  static constexpr int STAGNATION = STAGNATION_ROUNDS;
   const uint32_t* __restrict__ cor_ptr;
   const int4* __restrict__ cor_idx;
   const float4* __restrict__ cor_w;
@@ -618,9 +617,8 @@ struct InflationProblem : LabelStore {
   // The Sethian fallback produces trigger / back-step-child cycles on ordinary inputs (config 3: one pair oscillates for 27
   // of 41 rounds until the strict rule arms).  Arming the rule earlier (2-4 stagnant rounds) halves the round count but is
   // NOT neutral: on meshes with exact key ties (unjittered grids) the early strict rounds converge to a different label
-  // (fuzz seed 51 case 56, 1 vertex) -- so the engine's threshold stays, and the stagnant rounds are made cheap by the
-  // clean-candidate skip instead (only the oscillating pair is recomputed).
-  static constexpr int STAGNATION = STAGNATION_ROUNDS;
+  // (fuzz seed 51 case 56, 1 vertex) -- so the engine's threshold (STAGNATION_ROUNDS) stays, and the stagnant rounds are
+  // made cheap by the clean-candidate skip instead (only the oscillating pair is recomputed).
   uint32_t* last_eval; uint32_t* dirty_round; int skip_clean;
   // In strict rounds a label also depends on the round number, but only through a deferral: an evaluation that deferred
   // nothing rests on triggers that were stable, and a trigger that is re-labelled later marks its face neighbours dirty.
@@ -829,7 +827,6 @@ template <class S>
 struct DijkstraProblemT : TimeAlg {
   static constexpr bool HAS_GOAL_TIME = false;    // edge weights >= 0: vertices pop in potential order, the test on the value is exact
   static constexpr bool CAN_SKIP = false;
-  static constexpr int STAGNATION = STAGNATION_ROUNDS;
   const uint32_t* __restrict__ adj_ptr;
   const uint2* __restrict__ adj_nw;
   const float* __restrict__ cost;
