@@ -112,7 +112,7 @@ struct MeshState : RayCasterState {
   DeviceBuffer<uint32_t> d_repair_chg, d_repair_bits; DeviceBuffer<unsigned int> d_repair_log_n;
   DeviceBuffer<float> d_face_normals, d_vertex_normals; DeviceBuffer<uint8_t> d_border;
   DeviceBuffer<float> d_layer_costs, d_layer_combined, d_clearance; DeviceBuffer<uint8_t> d_layer_mask;
-  DeviceBuffer<float4> d_pos4, d_vn4; DeviceBuffer<uint32_t> d_nbr8;     // packed copies for k_layers<true>
+  DeviceBuffer<float4> d_pos4, d_vn4; DeviceBuffer<uint32_t> d_nbr8;     // packed copies for the prefetching layer walk
   DeviceBuffer<unsigned int> d_overflow;
   // device-resident result of the last single CVP plan (for mnb_cvp_backtrack)
   const uint32_t* last_pred = nullptr; const float* last_dir = nullptr; const int32_t* last_cut = nullptr;
@@ -167,9 +167,9 @@ struct mnb_ctx : MeshState {
   float delta = 0.3f; int cluster = -1 /* -1: whole-grid cooperative kernel for single plans */; int batch_cluster = 0 /* 0: chosen per call from the goal count */; int threads = 512;
   int grid_blocks_per_sm = 0;
   int infl_skip_clean = 1;     // clean-candidate skip of the inflation wave (mnb_debug_set_infl_skip(ctx, 0) turns it off)
-  int layers_smem = 5;         // neighbourhood walk of k_layers: 0 thread-local seen-set, 1 shared-memory seen-set, 2-4 prefetching walk (64 / 128 / 32
-                               // threads per CTA), 5-7 the same with the 16-bit seen-set (64 / 128 / 256), 8-9 its low-register builds.
-                               // Chosen per mesh by mnb_set_mesh unless fixed by mnb_debug_set_layers_smem.
+  int layers_walk = LAYERS_WALK_PF16;   // neighbourhood walk of k_layers: LAYERS_WALK_LOCAL (thread-local seen-set),
+                                        // LAYERS_WALK_PF32 / LAYERS_WALK_PF16 (prefetching walk, 32-bit / compact seen-set).
+                                        // Chosen per mesh by mnb_set_mesh unless fixed by mnb_debug_set_layers_smem.
   bool layers_explicit = false;
   uint32_t replan_pool_room = 0;   // level-pool words a resumed replan wave may add (mnb_debug_set_replan_pool_room; 0 = the pool's)
   int sweeps = -1;             // in-round sweeps of the whole-grid single plans (mnb_debug_set_sweeps); -1 = derived from the band width
@@ -419,11 +419,11 @@ static int32_t impl_set_mesh(mnb_ctx* ctx, uint32_t V, uint32_t F, const float* 
   }
   HostTopology& T = ctx->topo;
   if (!ctx->layers_explicit) {
-    // the compact seen-set of the layer walk (walk_pf16) holds ids within +-32767 of the centre's: a neighbourhood reaches a
-    // few edges out, so it pays when edges connect nearby ids (scan / Morton numbering); otherwise the 32-bit form
+    // the compact seen-set of the layer walk (SharedSeen<uint16_t>) holds ids within +-32767 of the centre's: a neighbourhood
+    // reaches a few edges out, so it pays when edges connect nearby ids (scan / Morton numbering); otherwise the 32-bit form
     uint32_t maxd = 0;
     for (size_t e = 0; e < (size_t)T.E; ++e) { const uint32_t a = T.edges[2 * e], b = T.edges[2 * e + 1]; maxd = std::max(maxd, a > b ? a - b : b - a); }
-    ctx->layers_smem = (maxd <= 8000u) ? 5 : 2;
+    ctx->layers_walk = (maxd <= 8000u) ? LAYERS_WALK_PF16 : LAYERS_WALK_PF32;
   }
   ctx->V = V; ctx->F = F; ctx->E = T.E; ctx->NC = T.cor_v1.size(); ctx->NA = T.vadj_nbr.size();
   const size_t NC = ctx->NC, NA = ctx->NA;
@@ -1260,41 +1260,22 @@ static int32_t impl_compute_layers(mnb_ctx* ctx, const mnb_layer_params* params,
   a.costs = o_costs; a.combined = o_combined; a.lethal_mask = o_mask;
   a.overflow = ctx->d_overflow;
   CK(cudaEventRecord(ctx->ev0, ctx->stream));
-  if (ctx->layers_smem) {
-    if (!ctx->d_pos4) {
-      CK(ctx->d_pos4.reserve(V)); CK(ctx->d_vn4.reserve(V)); CK(ctx->d_nbr8.reserve(8 * V));
-      MNB_LAUNCH(k_pack_layers, (ctx->V + 255) / 256, 256, 0, ctx->stream, (const float*)ctx->d_pos, (const float*)ctx->d_vertex_normals,
-                 (const uint32_t*)ctx->d_adj_ptr, (const uint32_t*)ctx->d_adj_nbr, ctx->V, ctx->d_pos4, ctx->d_vn4, ctx->d_nbr8);
-      CK(cudaGetLastError());
-    }
-    a.pos4 = ctx->d_pos4; a.vn4 = ctx->d_vn4; a.nbr8 = reinterpret_cast<const uint4*>(ctx->d_nbr8.p);
-    if (ctx->layers_smem == 8 || ctx->layers_smem == 9) {      // walk_pf16 compiled for more resident CTAs (fewer registers): 8 -> 64 x 12, 9 -> 128 x 6
-      const int T = ctx->layers_smem == 8 ? 64 : 128;
-      const size_t smem = (size_t)(2 * NB_HASH + LS_STACK) * T;
-      if (T == 64) { CK(cudaFuncSetAttribute(k_layers_pf16<64, 12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH((k_layers_pf16<64, 12>), (ctx->V + 63) / 64, 64, smem, ctx->stream, a); }
-      else { CK(cudaFuncSetAttribute(k_layers_pf16<128, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH((k_layers_pf16<128, 6>), (ctx->V + 127) / 128, 128, smem, ctx->stream, a); }
-    } else
-    if (ctx->layers_smem >= 5) {            // walk_pf16 (16-bit seen-set): 5 -> 64 threads per CTA, 6 -> 128, 7 -> 256
-      const int T = ctx->layers_smem == 5 ? 64 : (ctx->layers_smem == 6 ? 128 : 256);
-      const size_t smem = (size_t)(2 * NB_HASH + LS_STACK) * T;
-      if (T == 64) { CK(cudaFuncSetAttribute(k_layers_pf16<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH(k_layers_pf16<64>, (ctx->V + 63) / 64, 64, smem, ctx->stream, a); }
-      else if (T == 128) { CK(cudaFuncSetAttribute(k_layers_pf16<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH(k_layers_pf16<128>, (ctx->V + 127) / 128, 128, smem, ctx->stream, a); }
-      else { CK(cudaFuncSetAttribute(k_layers_pf16<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH(k_layers_pf16<256>, (ctx->V + 255) / 256, 256, smem, ctx->stream, a); }
-    } else
-    if (ctx->layers_smem >= 2) {            // walk_pf: 2 -> 64 threads per CTA, 3 -> 128, 4 -> 32
-      const int T = ctx->layers_smem == 2 ? 64 : (ctx->layers_smem == 3 ? 128 : 32);
-      const size_t smem = sizeof(uint32_t) * (size_t)(NB_HASH + LS_STACK) * T;
-      if (T == 64) { CK(cudaFuncSetAttribute(k_layers_pf<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH(k_layers_pf<64>, (ctx->V + 63) / 64, 64, smem, ctx->stream, a); }
-      else if (T == 128) { CK(cudaFuncSetAttribute(k_layers_pf<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH(k_layers_pf<128>, (ctx->V + 127) / 128, 128, smem, ctx->stream, a); }
-      else { CK(cudaFuncSetAttribute(k_layers_pf<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); MNB_LAUNCH(k_layers_pf<32>, (ctx->V + 31) / 32, 32, smem, ctx->stream, a); }
-    } else {
-    const size_t smem = sizeof(uint32_t) * (size_t)(NB_HASH + LS_STACK) * LS_THREADS;       // 88 KB: two CTAs per SM
-    CK(cudaFuncSetAttribute(k_layers<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    MNB_LAUNCH(k_layers<true>, (ctx->V + LS_THREADS - 1) / LS_THREADS, LS_THREADS, smem, ctx->stream, a);
-    }
-  } else {
-    MNB_LAUNCH(k_layers<false>, (ctx->V + 127) / 128, 128, 0, ctx->stream, a);
+  if (ctx->layers_walk != LAYERS_WALK_LOCAL && !ctx->d_pos4) {
+    CK(ctx->d_pos4.reserve(V)); CK(ctx->d_vn4.reserve(V)); CK(ctx->d_nbr8.reserve(8 * V));
+    MNB_LAUNCH(k_pack_layers, (ctx->V + 255) / 256, 256, 0, ctx->stream, (const float*)ctx->d_pos, (const float*)ctx->d_vertex_normals,
+               (const uint32_t*)ctx->d_adj_ptr, (const uint32_t*)ctx->d_adj_nbr, ctx->V, ctx->d_pos4, ctx->d_vn4, ctx->d_nbr8);
+    CK(cudaGetLastError());
   }
+  a.pos4 = ctx->d_pos4; a.vn4 = ctx->d_vn4; a.nbr8 = reinterpret_cast<const uint4*>(ctx->d_nbr8.p);
+  const auto launch = [&](void (*kern)(const LayerKernelArgs), int threads, size_t smem) -> int32_t {
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MNB_LAUNCH(kern, (ctx->V + threads - 1) / threads, threads, smem, ctx->stream, a);
+    return MNB_OK;
+  };
+  const int32_t rc = ctx->layers_walk == LAYERS_WALK_PF16 ? launch(k_layers<LAYERS_WALK_PF16>, PF_THREADS, PF_THREADS * SharedSeen<uint16_t>::BYTES)
+                     : ctx->layers_walk == LAYERS_WALK_PF32 ? launch(k_layers<LAYERS_WALK_PF32>, PF_THREADS, PF_THREADS * SharedSeen<uint32_t>::BYTES)
+                     : launch(k_layers<LAYERS_WALK_LOCAL>, LOCAL_THREADS, 0);
+  if (rc != MNB_OK) return rc;
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   CK(io.copy_back());
@@ -1408,7 +1389,10 @@ int32_t mnb_debug_set_sweeps(mnb_ctx* ctx, int32_t k) { if (!ctx || k < -1 || k 
 int32_t mnb_debug_set_replan_pool_room(mnb_ctx* ctx, uint32_t words) { if (!ctx) return MNB_E_ARG; ctx->replan_pool_room = words; return MNB_OK; }
 
 int32_t mnb_debug_set_infl_skip(mnb_ctx* ctx, int32_t on) { if (!ctx) return MNB_E_ARG; ctx->infl_skip_clean = on != 0; return MNB_OK; }
-int32_t mnb_debug_set_layers_smem(mnb_ctx* ctx, int32_t mode) { if (!ctx || mode < 0 || mode > 9) return MNB_E_ARG; ctx->layers_smem = mode; ctx->layers_explicit = true; return MNB_OK; }
+int32_t mnb_debug_set_layers_smem(mnb_ctx* ctx, int32_t mode) {
+  if (!ctx || (mode != LAYERS_WALK_LOCAL && mode != LAYERS_WALK_PF32 && mode != LAYERS_WALK_PF16)) return MNB_E_ARG;
+  ctx->layers_walk = mode; ctx->layers_explicit = true; return MNB_OK;
+}
 
 // test hooks (not part of the public header) of the single-plan CVP epilogue.  set: 0 (default) replays a vertex on its
 // ELL row where that covers it and hands the others to the CSR replay; 1 hands every vertex that is replayed at all (reached,

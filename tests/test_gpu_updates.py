@@ -254,12 +254,13 @@ def test_clean_candidate_skip_is_exact(api, oracle_mod, n, factor):
 
 
 def test_layers_shared_memory_variant_is_identical(api, oracle_mod):
-    """opt-in k_layers<true> (seen-set and stack of the neighbourhood walk in shared memory): same traversal order, so every
-    output is bit-identical to the default kernel, including on an irregular mesh whose hub overflows into the fallback"""
+    """the prefetching walks of k_layers (seen-set and stack in shared memory; mode 2: 32-bit ids, mode 5: the compact
+    16-bit form) against the thread-local walk (mode 0): same traversal order, so every output is bit-identical, including
+    on an irregular mesh whose hub overflows into the fallback; no other mode is accepted"""
     import ctypes as C
     from tests.util import delaunay_mesh
     # third mesh: a 200 x 200 terrain with randomly permuted vertex ids -- neighbour ids differ by up to 40 000, beyond the
-    # 16-bit codes of modes 5-7, so their per-vertex fallback runs next to the compact path
+    # 16-bit codes of mode 5, so its per-vertex fallback runs next to the compact path
     p3, f3 = mesh_case(200, True)
     perm = np.random.default_rng(9).permutation(p3.shape[0]).astype(np.uint32)
     q3 = np.empty_like(p3); q3[perm] = p3
@@ -271,8 +272,10 @@ def test_layers_shared_memory_variant_is_identical(api, oracle_mod):
         base = mm.computeLayers(P)
         P2 = api._lib.LayerParams.defaults(); P2.roughness_radius = 0.2; P2.ridge_radius = 0.45      # three separate walks
         b2 = mm.computeLayers(P2)
-        for mode in (1, 2, 3, 4, 5, 6, 7, 8, 9):   # 1: shared-memory seen-set; 2-4: the prefetching walk with 64 / 128 / 32 threads per CTA; 5-7: 16-bit seen-set, 64 / 128 / 256
-            mm.L.mnb_debug_set_layers_smem(mm._ctx, mode)
+        for mode in (-1, 1, 3, 4, 6, 7, 8, 9, 10):
+            assert mm.L.mnb_debug_set_layers_smem(mm._ctx, mode) == -1, mode      # MNB_E_ARG
+        for mode in (2, 5):
+            assert mm.L.mnb_debug_set_layers_smem(mm._ctx, mode) == 0
             got = mm.computeLayers(P)
             for k in list(api._lib.LAYER_NAMES) + ["combined"]:
                 assert (got[k].view(np.uint32) == base[k].view(np.uint32)).all(), (mode, k)

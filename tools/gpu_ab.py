@@ -3,7 +3,6 @@
 Prints, for each variant, kernel time + the bit-equality against the default kernel:
   * in-round sweeps / band width of the whole-grid single CVP plan (5 M), band width of the per-CTA batch (1 M, 2 goals
     per SM = one wave)
-  * k_layers<true> (shared-memory seen-set) on the 5 M mesh
   * the dynamic-obstacle cycle (inflation update, vector field, incremental layerChanged vs full re-install)"""
 import ctypes as C, sys, time
 import numpy as np
@@ -15,7 +14,6 @@ from mesh_navigation_b200.api import MeshMap, CVPMeshPlanner, InflationLayer
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 2240
 pos, faces = synth.grid_mesh(n, n, terrain=True)
 mm = MeshMap(pos, faces); ed = mm.edgeDistances(); vc = np.zeros(mm.V, np.float32); mm.setCosts(vc, ed)
-mm.L.mnb_debug_set_layers_smem.argtypes = [C.c_void_p, C.c_int32]
 c = synth.nearest_vertex(pos, [n * 0.05, n * 0.05, float(pos[:, 2].mean())])
 sf = int(2 * ((c // n) * (n - 1) + (c % n))); sp = pos[faces[sf]].mean(0).astype(np.float32)
 pl = CVPMeshPlanner(mm)
@@ -30,14 +28,7 @@ for (k, delta) in ((15, 1.8), (10, 1.2), (20, 2.4), (30, 3.6), (24, 1.8), (8, 1.
     print(f"[single {n}x{n}] sweeps={k} delta={delta}: kernel {best:.2f} ms rounds {g['rounds']} recomputes/V {g['recomputes']/mm.V:.2f} "
           f"dist!=default {int((g['dist'].view(np.uint32) != ref.view(np.uint32)).sum())}", flush=True)
 mm.L.mnb_debug_set_sweeps(mm._ctx, -1); mm.set_tuning(1.8, 0, 0)
-for smem in (0, 1, 0, 1):
-    mm.L.mnb_debug_set_layers_smem(mm._ctx, smem)
-    for it in range(2):
-        Ly = mm.computeLayers()
-    if smem == 0: base = Ly
-    same = all((Ly[k].view(np.uint32) == base[k].view(np.uint32)).all() for k in ("height_diff", "roughness", "ridge", "combined"))
-    print(f"[layers {n}x{n}] smem={smem}: kernel {Ly['kernel_ms']:.2f} ms, identical to default: {same}", flush=True)
-mm.L.mnb_debug_set_layers_smem(mm._ctx, 0)
+base = mm.computeLayers()
 # dynamic-obstacle cycle
 infl = InflationLayer(mm)
 static = base["combined"]; stat_le = np.where(base["lethal_mask"] != 0)[0]
