@@ -34,7 +34,9 @@
 #pragma once
 #include <cooperative_groups.h>
 #include <cstdint>
+#include <type_traits>
 
+#include "launch.cuh"
 #include "wavefront_math.cuh"
 
 namespace mnb {
@@ -368,7 +370,6 @@ __device__ __forceinline__ void group_sync(unsigned int* bar = nullptr) {
 template <int CAP_>
 struct StageT {
   static constexpr int CAP = CAP_;
-  static constexpr int SW_CAP = 1024;     // stage slots that take part in the in-round sweeps
   uint32_t buf[CAP];
   unsigned int n;
   unsigned int base;
@@ -376,35 +377,61 @@ struct StageT {
   unsigned int lo;
 };
 using Stage = StageT<3072>;
-// in-round sweeps (run_band_rounds_sub8<.., true>): per stage slot, the version of its vertex at the last evaluation
-// and a copy of its label; the per-sweep dirty list.  Lives in the shared memory of the whole-grid kernel only.
-struct SweepStage {
-  uint32_t seen[Stage::SW_CAP];
-  uint4 lab[Stage::SW_CAP];     // the slot vertex's own label (only its owner CTA writes it during a round)
-  uint16_t dl[Stage::SW_CAP];
+
+// The stage of the whole-grid kernels (k_cvp_grid, k_dijkstra_grid) together with the state of their in-round sweeps
+// (run_band_rounds_sub8<.., true>).  Its `cap` slots live in the kernel's dynamic shared memory, GRID_SLOT_BYTES each, and
+// `cap` is a kernel argument: the host sizes it from the device's opt-in shared memory (mnb_ctx::grid_slots).  Every slot
+// takes part in the sweeps, and the one-thread main pass walks a CTA's share of the list in chunks of `cap`.  Per slot:
+//   lab   the slot vertex's own label (only its owner CTA writes it during a round)
+//   buf   the staged vertex
+//   seen  the version of its vertex at the last evaluation
+//   gq    the main pass's queue of the candidates the one-thread evaluation leaves to the 8-lane one
+//   dl    the per-sweep dirty list (slot indices: cap <= 65535)
+struct GridStage {
+  unsigned int n;
+  unsigned int base;
+  unsigned int m_tau;
+  unsigned int lo;
   unsigned int dn[2];           // dirty-list length, double-buffered over sweeps
+  unsigned int cap;
+  // (the arrays in slot-size order, so that each stays aligned for any cap)
+  __device__ __forceinline__ uint4* lab() const { MNB_DYNAMIC_SMEM(s); return reinterpret_cast<uint4*>(s); }
+  __device__ __forceinline__ uint32_t* buf() const { MNB_DYNAMIC_SMEM(s); return reinterpret_cast<uint32_t*>(s + 16u * cap); }
+  __device__ __forceinline__ uint32_t* seen() const { MNB_DYNAMIC_SMEM(s); return reinterpret_cast<uint32_t*>(s + 20u * cap); }
+  __device__ __forceinline__ uint32_t* gq() const { MNB_DYNAMIC_SMEM(s); return reinterpret_cast<uint32_t*>(s + 24u * cap); }
+  __device__ __forceinline__ uint16_t* dl() const { MNB_DYNAMIC_SMEM(s); return reinterpret_cast<uint16_t*>(s + 28u * cap); }
 };
+constexpr unsigned int GRID_SLOT_BYTES = 16u + 4u + 4u + 4u + 2u;
+constexpr unsigned int GRID_SLOTS_MAX = 65535u;
 constexpr uint32_t SEEN_NEVER = 0xffffffffu;
 
-__device__ __forceinline__ void stage_put(Stage& st, unsigned int p, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
-  if (p < Stage::CAP) st.buf[p] = v;
+// slots and slot array of a stage
+template <int C> __device__ __forceinline__ unsigned int stage_cap(const StageT<C>&) { return (unsigned)C; }
+template <int C> __device__ __forceinline__ uint32_t* stage_buf(StageT<C>& st) { return st.buf; }
+__device__ __forceinline__ unsigned int stage_cap(const GridStage& st) { return st.cap; }
+__device__ __forceinline__ uint32_t* stage_buf(GridStage& st) { return st.buf(); }
+
+template <class S>
+__device__ __forceinline__ void stage_put(S& st, unsigned int p, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
+  if (p < stage_cap(st)) stage_buf(st)[p] = v;
   else list_next[atomicAdd(count_next, 1u)] = v;  // overflow: straight to global
 }
-__device__ __forceinline__ unsigned int stage_push(Stage& st, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
+template <class S>
+__device__ __forceinline__ unsigned int stage_push(S& st, uint32_t v, uint32_t* list_next, unsigned int* count_next) {
   const unsigned int p = atomicAdd(&st.n, 1u);
   stage_put(st, p, v, list_next, count_next);
   return p;
 }
 // same into slot p (reserved by the caller), and registers the slot for the in-round sweeps with the version its vertex had
 // at the last evaluation
-__device__ __forceinline__ void stage_put_seen(Stage& st, SweepStage& ss, unsigned int p, uint32_t v, uint32_t seen, const uint4& label_bits,
+__device__ __forceinline__ void stage_put_seen(GridStage& st, unsigned int p, uint32_t v, uint32_t seen, const uint4& label_bits,
                                                uint32_t* list_next, unsigned int* count_next) {
-  stage_put(st, p, v, list_next, count_next);
-  if (p < Stage::SW_CAP) { ss.seen[p] = seen; ss.lab[p] = label_bits; }
+  if (p < st.cap) { st.buf()[p] = v; st.seen()[p] = seen; st.lab()[p] = label_bits; }
+  else list_next[atomicAdd(count_next, 1u)] = v;  // overflow: straight to global
 }
-__device__ __forceinline__ void stage_push_seen(Stage& st, SweepStage& ss, uint32_t v, uint32_t seen, const uint4& label_bits,
+__device__ __forceinline__ void stage_push_seen(GridStage& st, uint32_t v, uint32_t seen, const uint4& label_bits,
                                                 uint32_t* list_next, unsigned int* count_next) {
-  stage_put_seen(st, ss, atomicAdd(&st.n, 1u), v, seen, label_bits, list_next, count_next);
+  stage_put_seen(st, atomicAdd(&st.n, 1u), v, seen, label_bits, list_next, count_next);
 }
 
 // an empty stage (thread 0 of the CTA)
@@ -427,7 +454,8 @@ template <class S>
 __device__ __forceinline__ void stage_flush(S& st, uint32_t* list_next, unsigned int* count_next,
                                             unsigned int* g_m_tau, unsigned int* g_lo) {
   __syncthreads();
-  const unsigned int n = st.n < (unsigned)S::CAP ? st.n : (unsigned)S::CAP;
+  const unsigned int cap = stage_cap(st);
+  const unsigned int n = st.n < cap ? st.n : cap;
   if (threadIdx.x == 0) {
     st.base = n ? atomicAdd(count_next, n) : 0u;
     if (st.m_tau != INF_BITS) atomicMin(g_m_tau, st.m_tau);
@@ -435,7 +463,8 @@ __device__ __forceinline__ void stage_flush(S& st, uint32_t* list_next, unsigned
   }
   __syncthreads();
   const unsigned int base = st.base;
-  for (unsigned int i = threadIdx.x; i < n; i += blockDim.x) list_next[base + i] = st.buf[i];
+  const uint32_t* buf = stage_buf(st);
+  for (unsigned int i = threadIdx.x; i < n; i += blockDim.x) list_next[base + i] = buf[i];
   __syncthreads();
   if (threadIdx.x == 0) stage_init(st);
   // no barrier needed here: the group barrier that follows every flush orders the reset
@@ -677,20 +706,21 @@ __device__ void run_band_rounds(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_
 // -----------------------------------------------------------------------------
 // STOP_ON_OVERFLOW (the resumed replan wave): the loop also ends once the level pool has overflowed -- the host discards
 // the labels and runs the whole wave, so rounds on truncated pop times (which need not settle) would only cost time.
-template <int CS, bool SW, class P, bool STOP_ON_OVERFLOW = false>
+// St: Stage, or GridStage with the in-round sweeps (SW).
+template <int CS, bool SW, class P, bool STOP_ON_OVERFLOW = false, class St>
 __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, uint32_t* list1, uint32_t* mark,
-                                     Stage& st, const float delta, const uint32_t gthreads, const uint32_t gtid,
+                                     St& st, const float delta, const uint32_t gthreads, const uint32_t gtid,
                                      const int has_robot, const uint32_t r0, const uint32_t r1, const uint32_t r2,
                                      const double goal_dist_offset, const volatile int* cancel_flag,
                                      const float band_end_init, const uint32_t max_rounds, const int n_sweeps_arg,
-                                     SweepStage* ss, const uint32_t n_vertices) {
+                                     const uint32_t n_vertices) {
+  static_assert(SW == std::is_same_v<St, GridStage>, "the in-round sweeps keep their state in the GridStage");
   const int n_sweeps = SW ? n_sweeps_arg : 0;
   // CVP on the whole grid: the main pass hands each candidate to ONE thread first (P::eval_plain, ~400 candidates per CTA
   // and round on the 5M terrain -- seven serial batches of the 64 a CTA holds on 8 lanes each) and queues the few it
   // cannot take for the 8-lane evaluation.  The sweeps keep the 8-lane form: ~65 dirty candidates per CTA and sweep are
   // one batch, and a thread walking its faces one by one takes longer than 8 lanes taking one face each.
   constexpr bool FAST = SW && P::PLAIN_FAST;
-  __shared__ uint32_t gq[FAST ? Stage::SW_CAP : 1];
   __shared__ unsigned int gq_n;
   if constexpr (FAST) { if (threadIdx.x == 0) gq_n = 0; __syncthreads(); }
   bool rescanned = false;
@@ -720,14 +750,14 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     // stagnation watch (see run_band_rounds)
     if (r > 0 && __float_as_uint(m_prev) != INF_BITS && !(lo_prev > lo_best)) { if (++stagnant >= STAGNATION_ROUNDS) prob.strict = 1; }
     else { stagnant = 0; if (lo_prev > lo_best) lo_best = lo_prev; }
-    // the sweeps work on the first SW_CAP stage slots of a CTA: on very long fronts (tens of millions of vertices) the
+    // the sweeps work on the stage slots of a CTA: on very long fronts (tens of millions of vertices) the
     // band is narrowed so that a CTA's share of the list still fits (group-uniform, exactness does not depend on it)
 #ifdef MNB_EMU_ACTIVE   // round trace on the CPU interpreter of the kernels (tests/emu, MNB_EMU_TRACE=1)
     if (gtid == 0 && getenv("MNB_EMU_TRACE")) fprintf(stderr, "[round %u] list %u m_prev %g lo_prev %g strict %d\n", r, n, m_prev, lo_prev, prob.strict);
 #endif
     float delta_r = delta;
     if constexpr (SW) {
-      const float fit = (float)nblk * (0.8f * (float)Stage::SW_CAP);
+      const float fit = (float)nblk * (0.8f * (float)stage_cap(st));
       if ((float)n > fit) delta_r = fmaxf(0.25f * delta, delta * fit / (float)n);
     }
     float band_end = lo_prev + delta_r;
@@ -749,7 +779,7 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
         const float tv = __uint_as_float(__ldcg(&prob.state[v]).y);
         if (tv > goal) {
           mark[v] = MARK_CAND_ACT;
-          if constexpr (SW) stage_push_seen(st, *ss, v, SEEN_NEVER, __ldcg(&prob.state[v]), list_n, &ctl->count[next]);
+          if constexpr (SW) stage_push_seen(st, v, SEEN_NEVER, __ldcg(&prob.state[v]), list_n, &ctl->count[next]);
           else stage_push(st, v, list_n, &ctl->count[next]);
           requeued = true;
         }
@@ -780,8 +810,8 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
         }
         my_lo = fminf(my_lo, nt.a1);
         if constexpr (SW) {
-          if (fresh) stage_push_seen(st, *ss, c, v0, prob.pack_label(c, nd, nt), list_n, &ctl->count[next]);
-          else if (changed) ss->lab[slot] = prob.pack_label(c, nd, nt);
+          if (fresh) stage_push_seen(st, c, v0, prob.pack_label(c, nd, nt), list_n, &ctl->count[next]);
+          else if (changed) st.lab()[slot] = prob.pack_label(c, nd, nt);
         } else {
           stage_push(st, c, list_n, &ctl->count[next]);
         }
@@ -803,14 +833,14 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
         if (ix.x != -1) {
           if (!prob.prefetch_marks) { mk1 = __ldcg(&mark[ix.x]); if (P::TWO_SOURCES) mk2 = __ldcg(&mark[ix.y]); }
           if (mk1 == MARK_NONE && prob.eligible((uint32_t)ix.x) && atomicCAS(&mark[ix.x], MARK_NONE, MARK_CAND) == MARK_NONE)
-            { if constexpr (SW) stage_push_seen(st, *ss, (uint32_t)ix.x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]); else stage_push(st, (uint32_t)ix.x, list_n, &ctl->count[next]); }
+            { if constexpr (SW) stage_push_seen(st, (uint32_t)ix.x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]); else stage_push(st, (uint32_t)ix.x, list_n, &ctl->count[next]); }
           if (P::TWO_SOURCES && mk2 == MARK_NONE && prob.eligible((uint32_t)ix.y) && atomicCAS(&mark[ix.y], MARK_NONE, MARK_CAND) == MARK_NONE)
-            { if constexpr (SW) stage_push_seen(st, *ss, (uint32_t)ix.y, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]); else stage_push(st, (uint32_t)ix.y, list_n, &ctl->count[next]); }
+            { if constexpr (SW) stage_push_seen(st, (uint32_t)ix.y, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]); else stage_push(st, (uint32_t)ix.y, list_n, &ctl->count[next]); }
         }
         if (j == 0 && deg > 8)
           prob.activate(c, [&](uint32_t x) {
             if (__ldcg(&mark[x]) == MARK_NONE && prob.eligible(x) && atomicCAS(&mark[x], MARK_NONE, MARK_CAND) == MARK_NONE)
-              { if constexpr (SW) stage_push_seen(st, *ss, x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]); else stage_push(st, x, list_n, &ctl->count[next]); }
+              { if constexpr (SW) stage_push_seen(st, x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]); else stage_push(st, x, list_n, &ctl->count[next]); }
           });
         if (j == 0) mark[c] = MARK_CAND_ACT;
       }
@@ -836,7 +866,10 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       const unsigned int q = qb + ((threadIdx.x & 31) >> 3);
       bool has = q < cnt_g;
       uint32_t c = 0;
-      if (has) c = queued ? gq[q] : __ldcg(&list_r[(size_t)q * nblk + blk]);
+      if (has) {
+        if constexpr (FAST) c = queued ? st.gq()[q] : __ldcg(&list_r[(size_t)q * nblk + blk]);
+        else c = __ldcg(&list_r[(size_t)q * nblk + blk]);
+      }
       // issue the independent loads of the candidate together: its label, its ELL row, its mark (and version)
       Label old = prob.load_label(has ? c : 0u);
       int4 ix = prob.load_row_idx(has ? c : 0u, j);
@@ -860,8 +893,10 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       constexpr unsigned FULL = 0xffffffffu;
       const uint32_t lane = threadIdx.x & 31u, lt = (1u << lane) - 1u;
       const bool fast_round = !prob.strict && !(has_robot && goal_b != INF_BITS);
-      for (unsigned int cb = 0; cb < cnt; cb += (unsigned)Stage::SW_CAP) {
-        const unsigned int ce = min(cnt, cb + (unsigned)Stage::SW_CAP);
+      const unsigned int cap = st.cap;
+      uint32_t* const gq = st.gq();
+      for (unsigned int cb = 0; cb < cnt; cb += cap) {
+        const unsigned int ce = min(cnt, cb + cap);
         for (unsigned int ib = cb + (threadIdx.x & ~31u); ib < ce; ib += blockDim.x) {      // warp-uniform trip count
           const unsigned int i = ib + lane;
           bool has = i < ce;
@@ -929,11 +964,11 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
           const unsigned int tot = __shfl_sync(FULL, incl, 31);
           if (tot) {
             unsigned int p = warp_reserve(&st.n, tot) + incl - mine;
-            if (done) stage_put_seen(st, *ss, p++, c, v0, nb, list_n, &ctl->count[next]);
+            if (done) stage_put_seen(st, p++, c, v0, nb, list_n, &ctl->count[next]);
             for (; won; won &= won - 1u) {
               const int b = __ffs(won) - 1;
               const int4 ix = prob.load_row_idx(c, (uint32_t)(b >> 1));
-              stage_put_seen(st, *ss, p++, (b & 1) ? (uint32_t)ix.y : (uint32_t)ix.x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]);
+              stage_put_seen(st, p++, (b & 1) ? (uint32_t)ix.y : (uint32_t)ix.x, SEEN_NEVER, state_inf(), list_n, &ctl->count[next]);
             }
           }
           const bool defer = has && !done;
@@ -965,19 +1000,22 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
     if (gtid == 0) { ctl->t_ph[0] += (unsigned long long)(tps - tp0); ctl->t_ph[2] += cnt; }
 #endif
     // sweep 0 appends to dn[0]: after an odd sweep count the previous round's last sweep left its count there
-    if constexpr (SW) if (threadIdx.x == 0) ss->dn[0] = 0;
+    if constexpr (SW) if (threadIdx.x == 0) st.dn[0] = 0;
     if constexpr (SW) for (int sw = 0; sw < n_sweeps; ++sw) {
 #ifdef MNB_GRID_TIMING
       const long long tq0 = clock64();
 #endif
       __syncthreads();                       // stage pushes / label-cache writes of the previous phase are visible
-      const unsigned int ns = min(st.n, (unsigned int)Stage::SW_CAP);
-      unsigned int* dcur = &ss->dn[sw & 1];
-      if (threadIdx.x == 0) ss->dn[(sw + 1) & 1] = 0;
-      for (unsigned int i = threadIdx.x; i < ns; i += blockDim.x) {
-        const uint32_t c = st.buf[i];
-        const uint32_t v0 = __ldcg(&prob.ver[c]);
-        if (v0 != ss->seen[i]) { ss->seen[i] = v0; ss->dl[atomicAdd(dcur, 1u)] = (uint16_t)i; }
+      const unsigned int ns = min(st.n, st.cap);
+      unsigned int* dcur = &st.dn[sw & 1];
+      if (threadIdx.x == 0) st.dn[(sw + 1) & 1] = 0;
+      {
+        const uint32_t* buf = st.buf(); uint32_t* seen = st.seen(); uint16_t* dl = st.dl();
+        for (unsigned int i = threadIdx.x; i < ns; i += blockDim.x) {
+          const uint32_t c = buf[i];
+          const uint32_t v0 = __ldcg(&prob.ver[c]);
+          if (v0 != seen[i]) { seen[i] = v0; dl[atomicAdd(dcur, 1u)] = (uint16_t)i; }
+        }
       }
       __syncthreads();
       const unsigned int dn = *dcur;
@@ -990,10 +1028,10 @@ __device__ void run_band_rounds_sub8(P& prob, GroupCtl* ctl, uint32_t* list0, ui
       for (unsigned int ib = (threadIdx.x >> 5) * 4u; ib < dn; ib += (blockDim.x >> 3)) {
         const unsigned int i = ib + ((threadIdx.x & 31) >> 3);
         const bool has = i < dn;
-        const uint32_t slot = has ? ss->dl[i] : 0u;
-        const uint32_t c = has ? st.buf[slot] : 0u;
+        const uint32_t slot = has ? st.dl()[i] : 0u;
+        const uint32_t c = has ? st.buf()[slot] : 0u;
         // own label from the CTA's cache, ELL row through L1: the source labels are the only L2 trip of the chain
-        const Label old = has ? prob.unpack_label(c, ss->lab[slot]) : prob.unpack_label(0u, state_inf());
+        const Label old = has ? prob.unpack_label(c, st.lab()[slot]) : prob.unpack_label(0u, state_inf());
         int4 ix = prob.load_row_idx(c, j);
         float4 w = prob.load_row_w(c, j);
         const uint32_t mk = __ldcg(&mark[c]);

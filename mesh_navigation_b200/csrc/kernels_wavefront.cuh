@@ -52,6 +52,7 @@ struct CvpKernelArgs {
   uint32_t max_rounds;
   int sweeps;                   // in-round sweeps of a single plan (0 = off, -1 = from the band width)
   float hop;                    // ~ one dependency hop in potential units (1.35 x mean edge weight)
+  uint32_t slots;               // k_cvp_grid: GridStage slots per CTA (in the tail padding: the struct keeps its size)
 };
 // the arguments of the matrix form of k_cvp_batch.  A type of its own rather than a field of CvpKernelArgs: the batch
 // kernels pass their arguments by reference to out-of-line functions, which copy them to the stack, so a larger
@@ -204,7 +205,7 @@ __global__ void __launch_bounds__(MNB_CVP_THREADS, MNB_CVP_MINBLOCKS) k_cvp(cons
   const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : prob.seed_max_d;
   run_band_rounds_sub8<CS, false, CvpEllProblem, RESUME>(prob, ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, has_robot,
                         rv[0], rv[1], rv[2], a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)),
-                        a.max_rounds, 0, nullptr, a.V);     // in-round sweeps are compiled into the whole-grid kernel only
+                        a.max_rounds, 0, a.V);     // in-round sweeps are compiled into the whole-grid kernel only
   group_sync<CS>();
   if (a.out_dist)
     for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
@@ -368,24 +369,25 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_
 // RESUME: as k_cvp<CS, true> (mnb_cvp_replan)
 template <bool RESUME = false>
 __global__ void __launch_bounds__(512, MNB_GRID_MINBLOCKS) k_cvp_grid(const CvpKernelArgs a) {
-  __shared__ Stage st;
-  __shared__ SweepStage sws;
+  __shared__ GridStage st;          // + a.slots x GRID_SLOT_BYTES of dynamic shared memory
   uint32_t g, gthreads, gtid;
   group_coords<0>(g, gthreads, gtid);
   GroupCtl* ctl = a.ws.ctl;
-  if (threadIdx.x == 0) { stage_init(st); sws.dn[0] = 0; sws.dn[1] = 0; }
+  if (threadIdx.x == 0) { stage_init(st); st.dn[0] = 0; st.dn[1] = 0; st.cap = a.slots; }
   __syncthreads();
   CvpEllProblem prob;
   uint32_t rv[3];
   cvp_single_setup<0, RESUME>(a, true, true, gthreads, gtid, prob, rv);
   const float delta = a.delta;      // not clamped to goal_dist_offset: the engine caps settling instead (settle_cap)
-  // in-round sweeps pay off once the band is several dependency hops deep; 12 were measured best on the 5M terrain
+  // in-round sweeps pay off once the band is several dependency hops deep.  On the 5 M terrain with 2048 GridStage slots
+  // and a 40 w band (29 hops; H100 80GB HBM3, 700 W): 12 / 18 / 24 / 32 / 48 sweeps took 39.3 / 35.7 / 34.6 / 34.9 / 36.2 ms
+  // (rounds 189 / 135 / 117 / 112 / 106), so at most 24
   int sweeps = a.sweeps;
-  if (sweeps < 0) sweeps = delta < 2.8f * a.hop ? 0 : min(12, (int)(delta / a.hop));
+  if (sweeps < 0) sweeps = delta < 2.8f * a.hop ? 0 : min(24, (int)(delta / a.hop));
   const float band_init = RESUME ? __uint_as_float(__ldcg(&ctl->lo[2])) : prob.seed_max_d;    // (see k_cvp)
   run_band_rounds_sub8<0, true, CvpEllProblem, RESUME>(prob, ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, a.robot_face >= 0,
                           rv[0], rv[1], rv[2], a.goal_dist_offset, a.cancel_flag, nextafterf(band_init, __uint_as_float(INF_BITS)), a.max_rounds,
-                          sweeps, &sws, a.V);
+                          sweeps, a.V);
   group_sync<0>(ctl->barrier);
   if (a.out_dist)
     for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
@@ -601,7 +603,7 @@ struct DijkstraKernelArgs {
   float* out_dist; uint32_t* out_pred;
   const int* cancel_flag;
   uint32_t max_rounds;
-  const uint4* ell_adj; int sweeps; float hop;   // whole-grid kernel only
+  const uint4* ell_adj; int sweeps; float hop; uint32_t slots;   // whole-grid kernel only (slots: see k_cvp_grid)
 };
 
 // The prologue of a single-plan Dijkstra wave (k_dijkstra, k_dijkstra_grid): the clearing pass (the sweep versions only for
@@ -875,11 +877,10 @@ __global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_dijk
 // Single Dijkstra plan on the whole GPU: 8 lanes per candidate (one edge each), wide band + in-round sweeps,
 // same engine instance as k_cvp_grid.
 __global__ void __launch_bounds__(512, 1) k_dijkstra_grid(const DijkstraKernelArgs a) {
-  __shared__ Stage st;
-  __shared__ SweepStage sws;
+  __shared__ GridStage st;          // + a.slots x GRID_SLOT_BYTES of dynamic shared memory
   uint32_t g, gthreads, gtid;
   group_coords<0>(g, gthreads, gtid);
-  if (threadIdx.x == 0) { stage_init(st); sws.dn[0] = 0; sws.dn[1] = 0; }
+  if (threadIdx.x == 0) { stage_init(st); st.dn[0] = 0; st.dn[1] = 0; st.cap = a.slots; }
   __syncthreads();
   DijkstraEllProblem prob;
   dijkstra_single_setup<0>(a, true, gthreads, gtid, prob);
@@ -888,9 +889,10 @@ __global__ void __launch_bounds__(512, 1) k_dijkstra_grid(const DijkstraKernelAr
   const uint32_t rv = has_robot ? (uint32_t)a.robot_vertex : 0xffffffffu;
   const float delta = a.delta;      // not clamped to goal_dist_offset: the engine caps settling instead (settle_cap)
   int sweeps = a.sweeps;
+  // (at most 15: with 2048 slots and a 40 w band on the 5 M terrain 15 / 24 / 36 sweeps took 11.1 / 11.7 / 12.9 ms)
   if (sweeps < 0) sweeps = delta < 2.8f * a.hop ? 0 : min(15, (int)(delta / a.hop));
   run_band_rounds_sub8<0, true>(prob, a.ws.ctl, a.ws.list0, a.ws.list1, a.ws.mark, st, delta, gthreads, gtid, has_robot, rv, rv, rv,
-                                a.goal_dist_offset, a.cancel_flag, 1e-30f, a.max_rounds, sweeps, &sws, a.V);
+                                a.goal_dist_offset, a.cancel_flag, 1e-30f, a.max_rounds, sweeps, a.V);
   group_sync<0>(a.ws.ctl->barrier);
   for (uint32_t v = gtid; v < a.V; v += gthreads) a.out_dist[v] = __uint_as_float(a.ws.state[v].x);
 }

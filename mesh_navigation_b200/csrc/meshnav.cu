@@ -37,6 +37,20 @@ constexpr double INFL_REPAIR_MAX_SHARE = 0.5;
 // default band width of the batched Dijkstra planner in mean edge weights: on the 1 M terrain with 1024 goals 1.5 w was
 // fastest of 1 - 10 w (DESIGN §5)
 constexpr float DIJKSTRA_BATCH_DELTA_W = 1.5f;
+// GridStage slots per CTA of the whole-grid single-plan kernels (k_cvp_grid, k_dijkstra_grid), fewer if the device's
+// opt-in shared memory per block holds fewer.  Measured on the 5 M bench plan (tools/gpu_sweep_slots.py; H100 80GB HBM3,
+// 700 W, 1980 MHz; median of 5 plans, L2 flushed): at the best band and sweep count of each, k_cvp_grid + epilogue took
+// 37.1 ms with 1024 slots (20 w, 12 sweeps), 34.6 ms with 2048 (40 w, 24), 35.1 ms with 3072 (60 w, 48), 35.9 ms with 4096
+// (40 w, 24) and 39.1 ms with 6144 (60 w, 48).  More slots take fewer rounds (117 at 2048, 75 at 3072), but the shared
+// memory they take (30 B per slot) comes out of the L1 that caches the ELL rows the sweeps read: at 20 w the same plan
+// costs 37.1 / 37.2 / 37.9 / 38.8 / 42.2 ms from 1024 to 6144 slots.  2048 slots (60 KB) is the trade-off.
+constexpr uint32_t GRID_SLOTS_DEFAULT = 2048;
+// single-plan band widths in mean edge weights w (install_weights): 40 w measured best for both kernels at 2048 slots
+// (CVP: 37.2 / 35.3 / 34.6 / 38.2 ms at 20 / 30 / 40 / 60 w with their best sweep counts; Dijkstra: 12.0 / 11.1 / 11.0 ms at
+// 25 / 40 / 60 w, where 60 w needs 24 sweeps and 40 w keeps the 15 of the sweep rule)
+constexpr float GRID_BAND_W = 40.0f;
+// static shared memory of the whole-grid kernels (GridStage's counters and the main pass's queue length) is far below this
+constexpr size_t GRID_STATIC_SMEM_ROOM = 1024;
 
 // ============================================================================
 // host side
@@ -166,6 +180,9 @@ struct mnb_ctx : MeshState {
   // tuning
   float delta = 0.3f; int cluster = -1 /* -1: whole-grid cooperative kernel for single plans */; int batch_cluster = 0 /* 0: chosen per call from the goal count */; int threads = 512;
   int grid_blocks_per_sm = 0;
+  uint32_t grid_slots = 0;     // GridStage slots per CTA of the whole-grid kernels (mnb_debug_set_sweep_slots); set by mnb_create
+  uint32_t grid_slots_max = 0; // as many as the device's opt-in shared memory per block holds (at most GRID_SLOTS_MAX)
+  size_t grid_smem_set[3] = {0, 0, 0};   // dynamic shared memory the three whole-grid kernels were last checked and set up for
   int infl_skip_clean = 1;     // clean-candidate skip of the inflation wave (mnb_debug_set_infl_skip(ctx, 0) turns it off)
   int layers_walk = LAYERS_WALK_PF16;   // neighbourhood walk of k_layers: LAYERS_WALK_LOCAL (thread-local seen-set),
                                         // LAYERS_WALK_PF32 / LAYERS_WALK_PF16 (prefetching walk, 32-bit / compact seen-set).
@@ -179,7 +196,7 @@ struct mnb_ctx : MeshState {
   float dijkstra_batch_delta = 0.18f;
   // The band widths above are potentials, i.e. multiples of the edge weights: unless the caller fixed them (mnb_set_tuning
   // with band_delta > 0) they follow the mean finite edge weight w of the installed weights -- 2.5 w for batches, 20 w for a
-  // single CVP plan, 25 w for a single Dijkstra plan, less on maps above ~12 M vertices, DIJKSTRA_BATCH_DELTA_W w for
+  // single CVP or Dijkstra plan (GRID_BAND_W), less on maps above ~9 M vertices, DIJKSTRA_BATCH_DELTA_W w for
   // Dijkstra batches (install_weights); one dependency hop is
   // ~1.35 w (the in-round sweeps are counted in hops).  On the 0.1 m bench meshes (w = 0.118) that is 0.3 / 2.4 / 3.0 m, the values
   // the kernels were tuned with.
@@ -352,6 +369,18 @@ int32_t mnb_create(int32_t device, mnb_ctx** out_ctx) {
   if (cudaSetDevice(device) != cudaSuccess) return MNB_E_CUDA;
   mnb_ctx* c = new mnb_ctx();
   c->device = device; c->sm_count = prop.multiProcessorCount;
+  {
+    int optin = 0;
+#ifdef MNB_EMU_ACTIVE
+    optin = 227 * 1024;         // (the interpreter has no device attributes; an H100's opt-in limit)
+#else
+    if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess) { delete c; return MNB_E_CUDA; }
+#endif
+    const size_t room = (size_t)optin > GRID_STATIC_SMEM_ROOM ? (size_t)optin - GRID_STATIC_SMEM_ROOM : 0;
+    c->grid_slots_max = (uint32_t)std::min<size_t>(room / GRID_SLOT_BYTES, GRID_SLOTS_MAX);
+    c->grid_slots = std::min(GRID_SLOTS_DEFAULT, c->grid_slots_max);
+    if (c->grid_slots == 0) { delete c; return MNB_E_CUDA; }
+  }
   if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return MNB_E_CUDA; }
   cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
   c->d_next_query.reserve(1);
@@ -512,16 +541,16 @@ static int32_t install_weights(mnb_ctx* ctx) {
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->w_mean = hs[1] > 0 ? (float)(hs[0] / hs[1]) : 0.0f;
   if (!ctx->delta_explicit && ctx->w_mean > 0) {
-    // Single plans: the band should hold about as many candidates as the grid has sweep slots (SM count x Stage::SW_CAP);
+    // Single plans: the band should hold about as many candidates as the grid has sweep slots (SM count x GridStage slots);
     // beyond that the in-round sweeps cannot follow and the band's rows fall out of the L2.  A front is ~3 sqrt(V) vertices
-    // long on a compact map and a hop is ~1.35 w deep.  5 M vertices: 20 w / 25 w (the values the kernels were tuned with);
-    // with 132 SMs the band narrows above ~9 M vertices (12 w at 25 M).
-    const float slots = (float)ctx->sm_count * (float)Stage::SW_CAP;
+    // long on a compact map and a hop is ~1.35 w deep.  5 M vertices: GRID_BAND_W for both planners; with 132 SMs and 2048
+    // slots the band narrows above ~9 M vertices (24 w at 25 M).
+    const float slots = (float)ctx->sm_count * (float)ctx->grid_slots;
     const float hops = slots / (3.0f * sqrtf((float)ctx->V));
     const float k = fmaxf(4.0f, 1.35f * hops);
     ctx->delta = 2.5f * ctx->w_mean;
-    ctx->grid_delta = fminf(20.0f, k) * ctx->w_mean;
-    ctx->dijkstra_grid_delta = fminf(25.0f, k) * ctx->w_mean;
+    ctx->grid_delta = fminf(GRID_BAND_W, k) * ctx->w_mean;
+    ctx->dijkstra_grid_delta = fminf(GRID_BAND_W, k) * ctx->w_mean;
     ctx->dijkstra_batch_delta = DIJKSTRA_BATCH_DELTA_W * ctx->w_mean;
   }
   ctx->costs_set = true;
@@ -697,14 +726,30 @@ static cudaError_t launch_cluster(void (*kern)(const KArgs), const KArgs& args, 
 
 // cooperative (grid-synchronising) launch of a kernel that takes one argument struct
 template <class KArgs>
-static cudaError_t launch_cooperative(void (*kern)(const KArgs), const KArgs& args, unsigned blocks, int threads, cudaStream_t stream) {
+static cudaError_t launch_cooperative(void (*kern)(const KArgs), const KArgs& args, unsigned blocks, int threads, cudaStream_t stream,
+                                      size_t smem = 0) {
 #ifdef MNB_EMU_ACTIVE
   (void)stream;
-  return emu::launch(kern, blocks, (unsigned)threads, (size_t)0, 1u, true, args);
+  return emu::launch(kern, blocks, (unsigned)threads, smem, 1u, true, args);
 #else
   void* kargs[] = {(void*)&args};
-  return cudaLaunchCooperativeKernel((const void*)kern, dim3(blocks), dim3(threads), kargs, 0, stream);
+  return cudaLaunchCooperativeKernel((const void*)kern, dim3(blocks), dim3(threads), kargs, smem, stream);
 #endif
+}
+
+// A whole-grid kernel (index k of mnb_ctx::grid_smem_set) with the dynamic shared memory of ctx->grid_slots GridStage slots:
+// allows that much, and checks that one CTA of `threads` still fits on an SM (the cooperative launch needs every CTA resident).
+template <class KArgs>
+static cudaError_t grid_kernel_smem(mnb_ctx* ctx, void (*kern)(const KArgs), int k, int threads, size_t& smem) {
+  smem = (size_t)ctx->grid_slots * GRID_SLOT_BYTES;
+  if (ctx->grid_smem_set[k] == smem) return cudaSuccess;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  int nb = 0;
+  if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, threads, smem)) != cudaSuccess) return e;
+  if (nb < 1) return cudaErrorInvalidValue;        // (no CTA fits)
+  ctx->grid_smem_set[k] = smem;
+  return cudaSuccess;
 }
 
 // free and total device memory (sizes the workspaces that are capped by memory)
@@ -877,13 +922,16 @@ template <bool RESUME>
 static int32_t launch_single_cvp(mnb_ctx* ctx, CvpKernelArgs a) {
   if (ctx->cluster == -1) {
     a.delta = ctx->grid_delta;
+    a.slots = ctx->grid_slots;
+    size_t smem = 0;
+    CK(grid_kernel_smem(ctx, k_cvp_grid<RESUME>, RESUME ? 1 : 0, ctx->threads, smem));
     if (ctx->grid_blocks_per_sm == 0) {
       int nb = 0;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_cvp_grid<false>, ctx->threads, 0));
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_cvp_grid<RESUME>, ctx->threads, smem));
       ctx->grid_blocks_per_sm = nb > MNB_GRID_MINBLOCKS ? MNB_GRID_MINBLOCKS : nb;
       if (nb <= 0) { ctx->err = "k_cvp_grid cannot be resident"; return MNB_E_CUDA; }
     }
-    CK(launch_cooperative(k_cvp_grid<RESUME>, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream));
+    CK(launch_cooperative(k_cvp_grid<RESUME>, a, (unsigned)(ctx->sm_count * ctx->grid_blocks_per_sm), ctx->threads, ctx->stream, smem));
   } else {
     const cudaError_t e = with_cluster_size<16>(ctx->cluster, [&](auto c) {
       constexpr int CS = decltype(c)::value;
@@ -1149,7 +1197,10 @@ static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_v
   const int cs = ctx->cluster;
   if (cs == -1) {   // single plan on the whole GPU (cooperative launch, one CTA per SM)
     a.delta = ctx->dijkstra_grid_delta; a.ell_adj = ctx->d_ell_adj; a.sweeps = ctx->sweeps; a.hop = ctx->w_mean > 0 ? 1.35f * ctx->w_mean : 0.16f;
-    e = launch_cooperative(k_dijkstra_grid, a, (unsigned)ctx->sm_count, 512, ctx->stream);
+    a.slots = ctx->grid_slots;
+    size_t smem = 0;
+    e = grid_kernel_smem(ctx, k_dijkstra_grid, 2, 512, smem);
+    if (e == cudaSuccess) e = launch_cooperative(k_dijkstra_grid, a, (unsigned)ctx->sm_count, 512, ctx->stream, smem);
   } else {
     e = with_cluster_size<16>(cs, [&](auto c) {
       constexpr int CS = decltype(c)::value;
@@ -1383,6 +1434,15 @@ static int32_t impl_locate(mnb_ctx* ctx, uint32_t n, const float* points, uint32
 
 // experiment knob (not part of the public header): in-round sweeps of the whole-grid single-plan kernel
 int32_t mnb_debug_set_sweeps(mnb_ctx* ctx, int32_t k) { if (!ctx || k < -1 || k > 64) return MNB_E_ARG; ctx->sweeps = k; return MNB_OK; }
+
+// test hook (not part of the public header): GridStage slots per CTA of the whole-grid single-plan kernels, 1 up to what the
+// device's shared memory holds (0 = the default).  The band widths derived from the slots follow at the next mnb_set_costs.
+int32_t mnb_debug_set_sweep_slots(mnb_ctx* ctx, int32_t n) {
+  if (!ctx || n < 0 || (uint32_t)n > ctx->grid_slots_max) return MNB_E_ARG;
+  ctx->grid_slots = n ? (uint32_t)n : std::min(GRID_SLOTS_DEFAULT, ctx->grid_slots_max);
+  ctx->grid_blocks_per_sm = 0;
+  return MNB_OK;
+}
 
 // test hook (not part of the public header): a resumed replan wave may add at most `words` level-pool words (0 = no limit
 // but the pool's), so that tests reach the whole-wave retry after a resumed wave ran out of pool
