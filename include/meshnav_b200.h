@@ -164,6 +164,37 @@ int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_face
                              float* out_dist /* [n][V] or NULL */, uint32_t* out_pred /* [n][V] or NULL */,
                              float* out_direction /* [n][V] or NULL */, int32_t* out_cutting_face /* [n][V] or NULL */);
 
+/* Batched CVP replanning after cost updates: the fleet's vector fields kept up to date without running every goal's wave
+ * again.  The outputs and the return code are bit-identical to mnb_cvp_batch_fields(ctx, n, seed_faces, seed_pos,
+ * cost_limit, ...) on the currently installed costs.  Any output may be NULL, not all of them.
+ * changed (n_changed entries, always a host pointer, any order, duplicates and unchanged vertices allowed) is the union
+ * of the changed sets of the mnb_update_vertex_costs calls since the last successful mnb_cvp_batch_replan on this
+ * context; the caller keeps it, as for mnb_cvp_replan.
+ * The context keeps a store of resident waves keyed by goal (seed face and the bits of the seed position).  A goal of
+ * this call resumes from its own T0 -- the earliest old pop time among the changed vertices and their face neighbours --
+ * when its wave is resident, the bits of cost_limit and the costs are those of the store (only mnb_update_vertex_costs
+ * since), its level pool is at most half full and every seed vertex pops before T0.  Any other goal runs a whole wave,
+ * which becomes resident if a slot is free.  Goals may be added, dropped or reordered between calls (matching is by
+ * key); resident goals absent from a call are released; duplicate goals share one wave and their rows are copies.
+ * A resident goal costs about 44 bytes per vertex (label, side arrays, level pool, pred / direction / cutting-face rows);
+ * the number of slots is capped by the device memory left after the workspace of the concurrent waves, and goals past
+ * the cap run whole waves on every call, still exact.  A resumed wave that overflows its level pool runs again as a
+ * whole wave.  mnb_get_stats sums rounds, recomputes and settled over the waves (a resumed goal counts its re-run tail).
+ * Nothing is written on MNB_E_ARG (n == 0, a NULL array that is needed, a changed id >= V), MNB_E_STATE (no costs),
+ * MNB_INVALID_START (a seed face >= F), MNB_E_NOMEM (not even one concurrent wave fits).  mnb_cancel: MNB_CANCELED,
+ * the rows are incomplete, the store is dropped and the next call runs whole waves.  mnb_set_mesh frees the store;
+ * mnb_set_costs and mnb_compute_edge_weights make it stale.  No other call disturbs it, and it disturbs neither
+ * mnb_cvp_replan's resident wave nor the last mnb_cvp result (mnb_cvp_backtrack, mnb_vector_map); it shares the
+ * wavefront workspace as mnb_cvp_batch_fields does, so the last inflation's labels are dropped.  The outputs follow
+ * mnb_set_pointer_mode. */
+int32_t mnb_cvp_batch_replan(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces /* n, host */,
+                             const float* seed_pos /* 3n, host */, double cost_limit,
+                             uint32_t n_changed, const uint32_t* changed /* host */,
+                             float* out_dist /* [n][V] or NULL */, uint32_t* out_pred /* [n][V] or NULL */,
+                             float* out_direction /* [n][V] or NULL */, int32_t* out_cutting_face /* [n][V] or NULL */);
+/* Frees the resident store of mnb_cvp_batch_replan (it can reach tens of GB); the next call runs whole waves. */
+int32_t mnb_cvp_batch_replan_release(mnb_ctx* ctx);
+
 /* Cost matrices: the cost from each of n seeds to each of m target vertices, e.g. from every candidate goal to every
  * robot of a fleet, without the [n][V] rows.  out[k][j] ([n][m] row-major) is bit-identical to
  * dist[k][target_vertices[j]] of mnb_dijkstra_batch (mnb_dijkstra_matrix) or of mnb_cvp_batch (mnb_cvp_matrix) with

@@ -52,6 +52,7 @@ EXPORTS = [
     "mnb_create", "mnb_destroy", "mnb_last_error", "mnb_set_pointer_mode", "mnb_stream", "mnb_set_mesh",
     "mnb_num_vertices", "mnb_num_faces", "mnb_num_edges", "mnb_get_edges", "mnb_get_edge_distances",
     "mnb_compute_edge_weights", "mnb_set_costs", "mnb_dijkstra", "mnb_dijkstra_batch", "mnb_cvp", "mnb_cvp_replan", "mnb_cvp_batch", "mnb_cvp_batch_fields",
+    "mnb_cvp_batch_replan", "mnb_cvp_batch_replan_release",
     "mnb_dijkstra_matrix", "mnb_cvp_matrix", "mnb_dijkstra_batch_repair", "mnb_inflate",
     "mnb_cancel", "mnb_get_stats", "mnb_set_tuning", "mnb_compute_layers", "mnb_get_vertex_normals", "mnb_vector_map", "mnb_cvp_backtrack", "mnb_locate",
     "mnb_update_vertex_costs", "mnb_get_costs", "mnb_max_combination_update", "mnb_avg_combination_update", "mnb_inflation_update", "mnb_inflation_repair",
@@ -91,6 +92,8 @@ def load():
     L.mnb_cvp_replan.restype = i32; L.mnb_cvp_replan.argtypes = [vp, u32, vp, i64, dbl, dbl, u32, vp, vp, vp, vp, vp]
     L.mnb_cvp_batch.restype = i32; L.mnb_cvp_batch.argtypes = [vp, u32, vp, vp, dbl, vp]
     L.mnb_cvp_batch_fields.restype = i32; L.mnb_cvp_batch_fields.argtypes = [vp, u32, vp, vp, dbl, vp, vp, vp, vp]
+    L.mnb_cvp_batch_replan.restype = i32; L.mnb_cvp_batch_replan.argtypes = [vp, u32, vp, vp, dbl, u32, vp, vp, vp, vp, vp]
+    L.mnb_cvp_batch_replan_release.restype = i32; L.mnb_cvp_batch_replan_release.argtypes = [vp]
     L.mnb_dijkstra_matrix.restype = i32; L.mnb_dijkstra_matrix.argtypes = [vp, u32, vp, u32, vp, dbl, vp]
     L.mnb_cvp_matrix.restype = i32; L.mnb_cvp_matrix.argtypes = [vp, u32, vp, vp, u32, vp, dbl, vp]
     L.mnb_dijkstra_batch_repair.restype = i32; L.mnb_dijkstra_batch_repair.argtypes = [vp, u32, vp, dbl, u32, vp, vp, vp]
@@ -126,6 +129,9 @@ def load():
     L.mnb_debug_set_cvp_epilogue.restype = i32; L.mnb_debug_set_cvp_epilogue.argtypes = [vp, i32]
     L.mnb_debug_get_epilogue_csr.restype = i32; L.mnb_debug_get_epilogue_csr.argtypes = [vp, C.POINTER(C.c_uint32)]
     L.mnb_debug_get_labels.restype = i32; L.mnb_debug_get_labels.argtypes = [vp, vp]
+    L.mnb_debug_set_batch_replan_slots.restype = i32; L.mnb_debug_set_batch_replan_slots.argtypes = [vp, i32]
+    L.mnb_debug_get_batch_replan_slots.restype = i32
+    L.mnb_debug_get_batch_replan_slots.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     L.mnb_debug_get_label_sides.restype = i32; L.mnb_debug_get_label_sides.argtypes = [vp, vp, vp, vp, u32]
     _lib = L
     return L

@@ -258,6 +258,27 @@ class MeshMap:
         return self._check(self.L.mnb_cvp_batch_fields(self._ctx, sf.size, _p(sf), _p(sp), float(cost_limit), opt(d_dist),
                                                        opt(d_pred), opt(d_dir), opt(d_cut)))
 
+    def cvp_batch_replan_dev(self, seed_faces, seed_pos, cost_limit, changed, d_dist: int, d_pred: int = 0, d_dir: int = 0,
+                             d_cut: int = 0) -> int:
+        """mnb_cvp_batch_replan with device outputs ([n,V] rows; 0 = not wanted); seeds and the changed vertices are host
+        values"""
+        sf = np.ascontiguousarray(seed_faces, dtype=np.uint32).reshape(-1)
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
+        ch = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        opt = lambda d: _p(d) if d else None
+        return self._check(self.L.mnb_cvp_batch_replan(self._ctx, sf.size, _p(sf), _p(sp), float(cost_limit), ch.size, _p(ch),
+                                                       opt(d_dist), opt(d_pred), opt(d_dir), opt(d_cut)))
+
+    def release_batch_replan(self):
+        """frees the resident waves of waveFrontReplanBatch (mnb_cvp_batch_replan_release)"""
+        self._check(self.L.mnb_cvp_batch_replan_release(self._ctx))
+
+    def batch_replan_slots(self):
+        """(resident slots of waveFrontReplanBatch, those that hold a wave the next call may resume) -- a test hook"""
+        n, v = C.c_uint32(0), C.c_uint32(0)
+        self._check(self.L.mnb_debug_get_batch_replan_slots(self._ctx, C.byref(n), C.byref(v)))
+        return n.value, v.value
+
     def dijkstra_matrix_dev(self, seed_vertices, target_vertices, cost_limit, d_out: int) -> int:
         """mnb_dijkstra_matrix with a device output ([n,m]); seeds and targets are host values"""
         sv = np.ascontiguousarray(seed_vertices, dtype=np.uint32).reshape(-1)
@@ -425,6 +446,26 @@ class CVPMeshPlanner:
         out = {k: (np.empty((sf.size, m.V), dtype=t) if k in want else None) for k, t in kinds.items()}
         rc = m._check(m.L.mnb_cvp_batch_fields(m._ctx, sf.size, _p(sf), _p(sp), float(self.cost_limit), _p(out["dist"]),
                                                _p(out["pred"]), _p(out["direction"]), _p(out["cutting_face"])))
+        return dict(outcome=rc, **out, **m.stats())
+
+    def waveFrontReplanBatch(self, seed_faces, seed_pos, changed=(), want=("dist", "pred", "direction", "cutting_face")):
+        """waveFrontPropagationBatchFields after layerChanged calls whose changed vertices are `changed` (their union since
+        the last waveFrontReplanBatch on this map): the same rows, bit for bit.  The map keeps the wave of each goal
+        (seed face and position) resident; a goal whose wave is resident and whose cost limit and costs are those of the
+        last call (only layerChanged since) resumes from the earliest moment the change can reach, the others run whole
+        waves.  Returns what waveFrontPropagationBatchFields returns; `settled` counts the re-run parts only."""
+        m = self.map
+        sf = np.ascontiguousarray(seed_faces, dtype=np.uint32).reshape(-1)
+        sp = np.ascontiguousarray(seed_pos, dtype=np.float32).reshape(-1, 3)
+        ch = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        kinds = dict(dist=np.float32, pred=np.uint32, direction=np.float32, cutting_face=np.int32)
+        unknown = set(want) - set(kinds)
+        if unknown:
+            raise ValueError(f"unknown outputs {sorted(unknown)}; choose from {list(kinds)}")
+        out = {k: (np.empty((sf.size, m.V), dtype=t) if k in want else None) for k, t in kinds.items()}
+        rc = m._check(m.L.mnb_cvp_batch_replan(m._ctx, sf.size, _p(sf), _p(sp), float(self.cost_limit), ch.size, _p(ch),
+                                               _p(out["dist"]), _p(out["pred"]), _p(out["direction"]),
+                                               _p(out["cutting_face"])))
         return dict(outcome=rc, **out, **m.stats())
 
     def costMatrix(self, seed_faces, seed_pos, target_vertices):

@@ -255,8 +255,9 @@ __device__ __noinline__ void batch_general_phase(const Args& a, const BatchGroup
 //     across the round barrier; (2) is one float per vertex written by its own last evaluation.  On the terrain 64 % of
 //     the evaluations of the plain round loop find nothing changed; this phase costs them ~25 thread-instructions.
 //   B (8 lanes per candidate): the evaluation proper, on the compacted work queue.
-// TARGETS (matrix form): the loop ends once every target of a.tg has settled, as in run_band_rounds.
-template <int CS, bool TARGETS = false, class Args>
+// TARGETS (matrix form): the loop ends once every target of a.tg has settled, as in run_band_rounds.  STOP_ON_OVERFLOW
+// (the batch replan): the loop also ends once the level pool has overflowed, as the resumed single plan's does.
+template <int CS, bool TARGETS = false, bool STOP_ON_OVERFLOW = false, class Args>
 __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const BatchGroup& G, uint32_t* list0, uint32_t* list1, BatchStage& st,
                                                       BatchWork& wk, const float delta, const uint32_t gthreads, const uint32_t gtid,
                                                       const SeedFace& sd, const float band_end_init) {
@@ -288,7 +289,7 @@ __device__ __forceinline__ void run_band_rounds_batch(const Args& a, const Batch
     const uint32_t* list_r = (r & 1) ? list1 : list0;
     uint32_t* list_n = (r & 1) ? list0 : list1;
     unsigned int* const count_next = &ctl->count[next];
-    band_advance<false>(ctl, gtid, r, INF_BITS, stop, a.cancel_flag);
+    band_advance<false, STOP_ON_OVERFLOW>(ctl, gtid, r, INF_BITS, stop, a.cancel_flag);
     const uint32_t buf_now = r & 1u, buf_prev = buf_now ^ 1u;      // re-labels of this round / of the previous round
     float my_mtau = INF, my_lo = INF;
     const unsigned int cnt = n > blk ? (n - blk + nblk - 1) / nblk : 0u;

@@ -473,22 +473,81 @@ __device__ __forceinline__ EvTime time_min_block(const TimeAlg& A, EvTime t) {
   return t;
 }
 
-// 1. per block: the earliest pop time over the changed vertices and their face neighbours (labels of the resident wave)
-__global__ void __launch_bounds__(256) k_replan_t0(const ReplanArgs a) {
-  const LabelStore S = replan_store(a);
+// The bodies the single replan (k_replan_*) and the batch replan (k_batch_replan_t0, k_cvp_batch_replan) share.
+// The earliest finite pop time of S over the changed vertices changed[i0], changed[i0 + stride], ... and their face
+// neighbours (time_never() if there is none).
+__device__ __forceinline__ EvTime replan_changed_min(const LabelStore& S, const uint32_t* changed, uint32_t n_changed, const uint32_t* cor_ptr,
+                                                     const int4* cor_idx, uint32_t i0, uint32_t stride) {
   EvTime best = time_never();
   auto consider = [&](uint32_t x) {
     const Label L = S.load_label(x);
     if (__float_as_uint(L.d) != INF_BITS && S.tless(L.t, best)) best = L.t;
   };
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n_changed; i += gridDim.x * blockDim.x) {
-    const uint32_t c = __ldg(&a.changed[i]);
+  for (uint32_t i = i0; i < n_changed; i += stride) {
+    const uint32_t c = __ldg(&changed[i]);
     consider(c);
-    for (uint32_t k = __ldg(&a.cor_ptr[c]), ke = __ldg(&a.cor_ptr[c + 1]); k < ke; ++k) {
-      const int4 ix = __ldg(&a.cor_idx[k]);
+    for (uint32_t k = __ldg(&cor_ptr[c]), ke = __ldg(&cor_ptr[c + 1]); k < ke; ++k) {
+      const int4 ix = __ldg(&cor_idx[k]);
       consider((uint32_t)ix.x); consider((uint32_t)ix.y);
     }
   }
+  return best;
+}
+// Does every vertex of the seed face sv pop before T0?  (Otherwise the wave runs whole.)
+__device__ __forceinline__ bool replan_seeds_before(const LabelStore& S, const uint32_t* sv, const EvTime& T0) {
+  bool ok = true;
+  for (int k = 0; k < 3; ++k) ok = ok && S.tless(S.load_label(__ldg(&sv[k])).t, T0);
+  return ok;
+}
+// The rollback of vertex v: a vertex that popped before T0 (and every seed vertex sv[]) stays settled with its label, pool
+// record included; every other one gets the state of a fresh wave.  Vertices that can never be fixed (invalid, cost >=
+// cost_limit) hold +inf and are reset with the rest.
+__device__ __forceinline__ void replan_rollback_vertex(const LabelStore& S, const uint32_t* sv, const EvTime& T0, uint32_t* mark, uint32_t v) {
+  const bool seed = v == __ldg(&sv[0]) || v == __ldg(&sv[1]) || v == __ldg(&sv[2]);
+  const Label L = S.load_label(v);
+  const bool keep = seed || (__float_as_uint(L.d) != INF_BITS && S.tless(L.t, T0));
+  if (keep) mark[v] = MARK_FIXED;
+  else { S.state[v] = state_inf(); mark[v] = MARK_NONE; }
+  S.chg[v] = 0u;
+}
+// The frontier test of vertex v after the rollback (every mark written, a barrier between): a vertex that may take a label
+// (as the wave's activation) and shares a face with a kept vertex is a first candidate -- in a fresh wave the kept labels
+// would have pulled it in.  It is appended to list0, counted in *count0.
+__device__ __forceinline__ void replan_frontier_vertex(const LabelStore& S, const uint32_t* sv, const uint32_t* cor_ptr, const int4* cor_idx,
+                                                       const float* cost, const uint8_t* invalid, double cost_limit, uint32_t* mark,
+                                                       uint32_t* list0, unsigned int* count0, uint32_t v) {
+  const uint32_t mv = __ldcg(&mark[v]);
+#ifdef MNB_EMU_ACTIVE
+  // the interpreter checks two invariants of the rollback: the seeds stay fixed, and a kept label's level stack names
+  // only kept vertices (levels are running maxima of the pop sequence, so they popped before; LabelStore::names relies on it)
+  if ((v == sv[0] || v == sv[1] || v == sv[2]) && mv != MARK_FIXED) { fprintf(stderr, "[replan] seed %u not fixed\n", v); abort(); }
+  if (mv == MARK_FIXED) {
+    const Label L = S.load_label(v);
+    for (uint32_t i = 1, n = S.levels_of(L.t); i <= n; ++i) {
+      uint32_t kb, id; S.level_of(L.t, i, kb, id);
+      if (id != v && mark[id] != MARK_FIXED) { fprintf(stderr, "[replan] kept label of %u names reset vertex %u\n", v, id); abort(); }
+    }
+  }
+#else
+  (void)S; (void)sv;
+#endif
+  if (mv != MARK_NONE) return;
+  if (!CvpProblem::eligible(v, cost, invalid, cost_limit)) return;
+  bool next_to_kept = false;
+  for (uint32_t k = __ldg(&cor_ptr[v]), ke = __ldg(&cor_ptr[v + 1]); k < ke && !next_to_kept; ++k) {
+    const int4 ix = __ldg(&cor_idx[k]);
+    next_to_kept = __ldcg(&mark[ix.x]) == MARK_FIXED || __ldcg(&mark[ix.y]) == MARK_FIXED;
+  }
+  if (next_to_kept) {
+    mark[v] = MARK_CAND;
+    list0[atomicAdd(count0, 1u)] = v;
+  }
+}
+
+// 1. per block: the earliest pop time over the changed vertices and their face neighbours (labels of the resident wave)
+__global__ void __launch_bounds__(256) k_replan_t0(const ReplanArgs a) {
+  const LabelStore S = replan_store(a);
+  EvTime best = replan_changed_min(S, a.changed, a.n_changed, a.cor_ptr, a.cor_idx, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
   best = time_min_block(S, best);
   if (threadIdx.x == 0) time_put(a.t0 + REPLAN_T0_WORDS + 6 * blockIdx.x, best);
 }
@@ -518,16 +577,13 @@ __global__ void __launch_bounds__(256) k_replan_t0_final(const ReplanArgs a, uin
     }
     if (all && S.tless(late, best)) best = late;
   }
-  bool ok = true;
-  for (int k = 0; k < 3; ++k) ok = ok && S.tless(S.load_label(__ldg(&a.faces[3 * (size_t)a.seed_face + k])).t, best);
+  const bool ok = replan_seeds_before(S, a.faces + 3 * (size_t)a.seed_face, best);
   time_put(a.t0, best);
   a.t0[6] = ok ? 1u : 0u;
 }
 
-// 3. the rollback: a vertex that popped before T0 (and every seed) stays settled with its label, pool record included;
-//    every other one gets the state of a fresh wave.  Vertices that can never be fixed (invalid, cost >= cost_limit) hold
-//    +inf and are reset with the rest.  The group's control block is reset for the round loop with the band at T0; the
-//    level pool keeps its records and allocation continues from its top.
+// 3. the rollback (replan_rollback_vertex).  The group's control block is reset for the round loop with the band at T0;
+//    the level pool keeps its records and allocation continues from its top.
 __global__ void __launch_bounds__(256) k_replan_rollback(const ReplanArgs a) {
   const LabelStore S = replan_store(a);
   const EvTime T0 = time_get(a.t0);
@@ -540,47 +596,233 @@ __global__ void __launch_bounds__(256) k_replan_rollback(const ReplanArgs a) {
     ctl->pool_top = top;
   }
   if (v >= a.V) return;
-  const uint32_t* sv = a.faces + 3 * (size_t)a.seed_face;
-  const bool seed = v == __ldg(&sv[0]) || v == __ldg(&sv[1]) || v == __ldg(&sv[2]);
-  const Label L = S.load_label(v);
-  const bool keep = seed || (__float_as_uint(L.d) != INF_BITS && S.tless(L.t, T0));
-  if (keep) a.ws.mark[v] = MARK_FIXED;
-  else { a.ws.state[v] = state_inf(); a.ws.mark[v] = MARK_NONE; }
-  a.ws.chg[v] = 0u;
+  replan_rollback_vertex(S, a.faces + 3 * (size_t)a.seed_face, T0, a.ws.mark, v);
   a.ws.ver[v] = 0u;
 }
 
-// 4. the first candidates: the vertices that may take a label (as k_cvp_grid's activation) and share a face with a kept
-//    vertex -- in a fresh wave the kept labels would have pulled them in
+// 4. the first candidates (replan_frontier_vertex)
 __global__ void __launch_bounds__(256) k_replan_frontier(const ReplanArgs a) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= a.V) return;
-  uint32_t* mark = a.ws.mark;
-  const uint32_t mv = __ldcg(&mark[v]);
-#ifdef MNB_EMU_ACTIVE
-  // the interpreter checks two invariants of the rollback: the seeds stay fixed, and a kept label's level stack names
-  // only kept vertices (levels are running maxima of the pop sequence, so they popped before; LabelStore::names relies on it)
-  const uint32_t* sv = a.faces + 3 * (size_t)a.seed_face;
-  if ((v == sv[0] || v == sv[1] || v == sv[2]) && mv != MARK_FIXED) { fprintf(stderr, "[replan] seed %u not fixed\n", v); abort(); }
-  if (mv == MARK_FIXED) {
-    const LabelStore S = replan_store(a);
-    const Label L = S.load_label(v);
-    for (uint32_t i = 1, n = S.levels_of(L.t); i <= n; ++i) {
-      uint32_t kb, id; S.level_of(L.t, i, kb, id);
-      if (id != v && mark[id] != MARK_FIXED) { fprintf(stderr, "[replan] kept label of %u names reset vertex %u\n", v, id); abort(); }
+  replan_frontier_vertex(replan_store(a), a.faces + 3 * (size_t)a.seed_face, a.cor_ptr, a.cor_idx, a.cost, a.invalid, a.cost_limit, a.ws.mark,
+                         a.ws.list0, &a.ws.ctl->count[0], v);
+}
+
+// ============================================================================
+// Batch replan (mnb_cvp_batch_replan): full-field waves of many goals resume from their own T0 (DESIGN §4, "Batch
+// replan").  Without a goal cutoff, T0 is the earliest old pop time in the closed 1-rings of the changed vertices.  The
+// resident waves live in slots, one device allocation each; the host uploads one BatchReplanGoal per distinct goal.
+// ============================================================================
+// One resident slot: the wave's labels and side arrays, its pred / dir / cut rows and its level pool, then a 16-byte
+// header (the pool top after the wave) -- 36 bytes per vertex, the pool's 4 * pool_cap bytes and the header.
+struct ReplanSlot {
+  uint4* state; uint32_t* ext; uint32_t* root; uint32_t* pred; float* dir; int32_t* cut; uint32_t* pool; uint32_t* pool_top;
+};
+__host__ __device__ __forceinline__ size_t replan_slot_bytes(uint32_t V, uint32_t pool_cap) {
+  return (size_t)V * (sizeof(uint4) + 5 * sizeof(uint32_t)) + (size_t)pool_cap * sizeof(uint32_t) + 16;
+}
+__device__ __forceinline__ ReplanSlot replan_slot(uint8_t* base, uint32_t V, uint32_t pool_cap) {
+  ReplanSlot s;
+  s.state = reinterpret_cast<uint4*>(base);
+  uint32_t* w = reinterpret_cast<uint32_t*>(base + (size_t)V * sizeof(uint4));
+  s.ext = w; s.root = w + V; s.pred = w + 2 * (size_t)V; s.dir = reinterpret_cast<float*>(w + 3 * (size_t)V);
+  s.cut = reinterpret_cast<int32_t*>(w + 4 * (size_t)V); s.pool = w + 5 * (size_t)V; s.pool_top = s.pool + pool_cap;
+  return s;
+}
+
+// one distinct goal of a call (q: its index in the call's seed arrays), built by the host
+struct BatchReplanGoal {
+  uint8_t* slot;                // its resident slot, or null: the wave runs whole in the workspace
+  uint32_t row;                 // the caller's row it writes (the host copies it to the rows of duplicate goals)
+  uint32_t resume;              // 1 when uploaded: the slot holds this goal's wave of the same costs and cost limit.
+                                // k_batch_replan_t0 leaves it at 1 only if the wave can resume.
+  uint32_t t0[6];               // T0 (k_batch_replan_t0)
+  unsigned int chunks_done;     // k_batch_replan_t0's finished blocks of this goal (0 when uploaded)
+};
+
+struct BatchReplanT0Args {
+  uint32_t V, pool_cap;
+  const uint32_t* faces; const uint32_t* cor_ptr; const int4* cor_idx;
+  BatchReplanGoal* goals; const uint32_t* seed_faces;
+  const uint32_t* changed; uint32_t n_changed;   // device, any order, duplicates allowed
+  uint32_t chunks;              // blocks per goal: block b serves goal b / chunks
+  uint32_t* minima;             // [goals][chunks] pop times (6 words)
+};
+
+// the label store of a batch wave's labels (chg and the pool top: the group's; k_batch_replan_t0 only reads the labels)
+__device__ __forceinline__ LabelStore batch_store(uint4* state, uint32_t* ext, uint32_t* root, uint32_t* pool, uint32_t pool_cap, uint32_t* chg,
+                                                  GroupCtl* ctl) {
+  LabelStore S;
+  S.state = state; S.root_arr = root; S.ext_arr = ext; S.chg = chg; S.pool = pool; S.pool_w = pool; S.pool_cap = pool_cap;
+  S.pool_top = ctl ? &ctl->pool_top : nullptr; S.pool_overflow = ctl ? &ctl->pool_overflow : nullptr;
+  return S;
+}
+
+// T0 of every goal that may resume, in one launch over (goal, chunk of the changed list): each block reduces its chunk;
+// the last block of a goal reduces the chunk minima and sets the resume flag -- every seed pops before T0 and the slot's
+// level pool is at most half full.  No changed vertex: T0 is "never", and the resumed wave re-runs nothing.
+__global__ void __launch_bounds__(256) k_batch_replan_t0(const BatchReplanT0Args a) {
+  const uint32_t q = blockIdx.x / a.chunks, chunk = blockIdx.x % a.chunks;
+  BatchReplanGoal* gq = a.goals + q;
+  if (!gq->resume) return;                                       // (block-uniform: a host value)
+  const ReplanSlot sl = replan_slot(gq->slot, a.V, a.pool_cap);
+  const LabelStore S = batch_store(sl.state, sl.ext, sl.root, sl.pool, a.pool_cap, nullptr, nullptr);
+  EvTime best = replan_changed_min(S, a.changed, a.n_changed, a.cor_ptr, a.cor_idx, chunk * blockDim.x + threadIdx.x, a.chunks * blockDim.x);
+  best = time_min_block(S, best);
+  __shared__ bool last;
+  if (threadIdx.x == 0) {
+    time_put(a.minima + 6 * (size_t)blockIdx.x, best);
+    __threadfence();                                             // the minimum before the count that publishes it
+    last = atomicAdd(&gq->chunks_done, 1u) == a.chunks - 1;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0 || !last) return;
+  __threadfence();
+  for (uint32_t b = 0; b < a.chunks; ++b) {
+    const EvTime u = time_get(a.minima + 6 * ((size_t)q * a.chunks + b));
+    if (S.tless(u, best)) best = u;
+  }
+  time_put(gq->t0, best);
+  const bool room = __ldcg(sl.pool_top) <= a.pool_cap / 2;
+  gq->resume = room && replan_seeds_before(S, a.faces + 3 * (size_t)a.seed_faces[q], best) ? 1u : 0u;
+}
+
+struct CvpBatchReplanArgs : CvpKernelArgs {
+  const BatchReplanGoal* goals; // [n_queries]
+  uint32_t pool_room;           // level-pool words a resumed wave may add (mnb_debug_set_replan_pool_room; 0 = the pool's)
+};
+
+// The rollback and the frontier of a resumed goal (seed face sv) on the group's labels G (a slot), then the control block
+// for the round loop with the band at T0 and the slot's pool top.  Called by every thread of the group; ends with a group
+// barrier.  Out of line, as the batch kernel's other once-per-wave work.
+template <int CS>
+__device__ __noinline__ void batch_replan_rollback(const CvpBatchReplanArgs& a, const BatchGroup& G, uint32_t* list0, const uint32_t* sv,
+                                                   const EvTime& T0, const uint32_t* pool_top, uint32_t gthreads, uint32_t gtid) {
+  const LabelStore S = batch_store(G.state, G.ext_arr, G.root_arr, G.pool, G.pool_cap, G.chg, G.ctl);
+  for (uint32_t v = gtid; v < a.V; v += gthreads) {
+    replan_rollback_vertex(S, sv, T0, G.mark, v);
+    G.skipw[v] = make_uint4(INF_BITS, INF_BITS, 0u, 0u);
+  }
+  if (gtid == 0) {
+    ctl_reset(G.ctl, 0u, T0.a1);
+    G.ctl->pool_top = __ldcg(pool_top);
+  }
+  group_sync<CS>();
+  for (uint32_t v = gtid; v < a.V; v += gthreads)
+    replan_frontier_vertex(S, sv, a.cor_ptr, a.cor_idx, a.cost, a.invalid, a.cost_limit, G.mark, list0, &G.ctl->count[0], v);
+  group_sync<CS>();
+}
+
+// The clearing pass and the seeding of a whole wave for goal q (as k_cvp_batch's); retry: the goal's resumed wave
+// overflowed the level pool, and the flag is cleared (after the barrier of the clearing pass: every thread of the group
+// has read it).  Called by every thread of the group; ends with a group barrier.
+template <int CS>
+__device__ __noinline__ void batch_replan_seed(const CvpBatchReplanArgs& a, const BatchGroup& G, uint32_t* list0, uint32_t q, bool retry,
+                                               uint32_t gthreads, uint32_t gtid) {
+  for (uint32_t v = gtid; v < a.V; v += gthreads) { G.state[v] = state_inf(); G.mark[v] = MARK_NONE; G.chg[v] = 0u; G.skipw[v] = make_uint4(INF_BITS, INF_BITS, 0u, 0u); }
+  group_sync<CS>();
+  if (gtid == 0) {
+    if (retry) G.ctl->pool_overflow = 0u;
+    const CvpSeeds cs = cvp_seeds(a.faces, a.pos, a.cost, a.invalid, a.cost_limit, a.seed_faces[q], a.seed_pos + 3 * (size_t)q);
+    CvpEllProblem prob;
+    batch_make_problem(a, G, cs, 0, prob);
+    seed_wave(prob, G.ctl, G.mark, list0, cs.s, cs.d, 3, cs.seed_min);
+  }
+  group_sync<CS>();
+}
+
+// The epilogue of goal q into pred / dir / cut (any may be null).  TAIL (a resumed wave): the kept vertices (MARK_FIXED)
+// are skipped -- they popped before T0, so none of their faces changed and their sources popped before them: their
+// entries in the slot's rows are still exact.
+__device__ __noinline__ void batch_replan_epilogue(const CvpKernelArgs& a, const BatchGroup& G, uint32_t q, uint32_t* pred, float* dir, int32_t* cut,
+                                                   bool tail, uint32_t gthreads, uint32_t gtid) {
+  const uint32_t sf = a.seed_faces[q];
+  CvpProblem prob;
+  cvp_epilogue_problem(a, G.state, G.ext_arr, G.root_arr, G.chg, G.pool, G.ctl, sf, a.seed_pos + 3 * (size_t)q, ev_normal(__uint_as_float(INF_BITS), 0u),
+                       pred, dir, cut, prob);
+  for (uint32_t v = gtid; v < a.V; v += gthreads)
+    if (!(tail && __ldcg(&G.mark[v]) == MARK_FIXED))
+      cvp_epilogue_vertex<false>(prob, a.ell_idx, a.ell_w, G.ctl, sf, __uint_as_float(INF_BITS), v, [](uint32_t) {});
+}
+
+// The batch replan: k_cvp_batch<CS, true> over the distinct goals of a.goals.  A goal with a slot keeps its labels, side
+// arrays, level pool and rows there; marks, chg, skipw and the lists are the group's workspace, as for a goal without
+// one.  A goal whose flag k_batch_replan_t0 left raised resumes from T0: rollback and frontier, the round loop with the band
+// just above T0 (stopping if the level pool overflows; then the goal runs again as a whole wave from an empty pool), and
+// the epilogue of the re-run tail alone.  Every other goal runs a whole wave.  No goal is taken once the cancel flag is set.
+template <int CS>
+__global__ void __launch_bounds__(MNB_BATCH_THREADS, MNB_BATCH_MINBLOCKS) k_cvp_batch_replan(const CvpBatchReplanArgs a) {
+  __shared__ BatchStage st;
+  __shared__ BatchWork wk;
+  uint32_t g, gthreads, gtid;
+  group_coords<CS>(g, gthreads, gtid);
+  const uint32_t V = a.V;
+  BatchGroup W;
+  W.state = a.ws.state + (size_t)g * V; W.root_arr = a.ws.root + (size_t)g * V; W.ext_arr = a.ws.ext + (size_t)g * V;
+  W.chg = a.ws.chg + (size_t)g * V; W.mark = a.ws.mark + (size_t)g * V; W.pool = a.ws.pool + (size_t)g * a.ws.pool_cap;
+  W.pool_cap = a.ws.pool_cap; W.ctl = a.ws.ctl + g; W.skipw = a.ws.skipw + (size_t)g * V;
+  uint32_t* list0 = a.ws.list0 + (size_t)g * V;
+  uint32_t* list1 = a.ws.list1 + (size_t)g * V;
+  GroupCtl* ctl = W.ctl;
+  if (threadIdx.x == 0) { stage_init(st); wk.n = 0; wk.ns = 0; }
+  __syncthreads();
+  for (;;) {
+    if (gtid == 0) ctl->query = (a.cancel_flag && *(const volatile int*)a.cancel_flag) ? a.n_queries : atomicAdd(a.next_query, 1u);
+    group_sync<CS>();
+    const uint32_t q = __ldcg(&ctl->query);
+    if (q >= a.n_queries) break;
+    const BatchReplanGoal* gq = a.goals + q;
+    uint8_t* const slot_base = gq->slot;
+    BatchGroup G = W;
+    ReplanSlot sl{};
+    if (slot_base) {
+      sl = replan_slot(slot_base, V, a.ws.pool_cap);
+      G.state = sl.state; G.ext_arr = sl.ext; G.root_arr = sl.root; G.pool = sl.pool;
     }
-  }
-#endif
-  if (mv != MARK_NONE) return;
-  if (!CvpProblem::eligible(v, a.cost, a.invalid, a.cost_limit)) return;
-  bool next_to_kept = false;
-  for (uint32_t k = __ldg(&a.cor_ptr[v]), ke = __ldg(&a.cor_ptr[v + 1]); k < ke && !next_to_kept; ++k) {
-    const int4 ix = __ldg(&a.cor_idx[k]);
-    next_to_kept = __ldcg(&mark[ix.x]) == MARK_FIXED || __ldcg(&mark[ix.y]) == MARK_FIXED;
-  }
-  if (next_to_kept) {
-    mark[v] = MARK_CAND;
-    a.ws.list0[atomicAdd(&a.ws.ctl->count[0], 1u)] = v;
+    const SeedFace sd = cvp_seeds(a.faces, a.pos, a.cost, a.invalid, a.cost_limit, a.seed_faces[q], a.seed_pos + 3 * (size_t)q);
+    // (a pool overflow of an earlier goal of the group fails the call: its goals then run whole, and nothing is retried)
+    bool resume = slot_base && gq->resume && !__ldcg(&ctl->pool_overflow), retry = false;
+    for (;;) {
+      float band_init;
+      if (resume) {
+        const EvTime T0 = time_get(gq->t0);
+        batch_replan_rollback<CS>(a, G, list0, a.faces + 3 * (size_t)a.seed_faces[q], T0, sl.pool_top, gthreads, gtid);
+        if (a.pool_room) G.pool_cap = min(G.pool_cap, __ldcg(&ctl->pool_top) + a.pool_room);
+        band_init = T0.a1;
+      } else {
+        batch_replan_seed<CS>(a, G, list0, q, retry, gthreads, gtid);
+        band_init = sd.seed_max;
+      }
+      run_band_rounds_batch<CS, false, true>(a, G, list0, list1, st, wk, a.delta, gthreads, gtid, sd, nextafterf(band_init, __uint_as_float(INF_BITS)));
+      group_sync<CS>();
+      if (!resume || !__ldcg(&ctl->pool_overflow)) break;
+      // the resumed wave ran out of level pool: the goal runs again as a whole wave from an empty pool (seed_wave resets
+      // the pool top)
+      resume = false; retry = true;
+      G.pool_cap = a.ws.pool_cap;
+    }
+    const size_t row = (size_t)gq->row * V;
+    uint32_t* const o_pred = a.out_pred ? a.out_pred + row : nullptr;
+    float* const o_dir = a.out_dir ? a.out_dir + row : nullptr;
+    int32_t* const o_cut = a.out_cut ? a.out_cut + row : nullptr;
+    if (slot_base) {
+      // the slot's rows are completed (the re-run tail, or every vertex), then copied to the caller's
+      batch_replan_epilogue(a, G, q, sl.pred, sl.dir, sl.cut, resume, gthreads, gtid);
+      group_sync<CS>();
+      for (uint32_t v = gtid; v < V; v += gthreads) {
+        if (o_pred) o_pred[v] = __ldcg(&sl.pred[v]);
+        if (o_dir) o_dir[v] = __ldcg(&sl.dir[v]);
+        if (o_cut) o_cut[v] = __ldcg(&sl.cut[v]);
+      }
+      if (gtid == 0) *sl.pool_top = ctl->pool_top;
+    } else if (o_pred || o_dir || o_cut) {
+      batch_replan_epilogue(a, G, q, o_pred, o_dir, o_cut, false, gthreads, gtid);
+    }
+    if (a.out_dist) {
+      float* od = a.out_dist + row;
+      for (uint32_t v = gtid; v < V; v += gthreads) od[v] = __uint_as_float(__ldcg(&G.state[v]).x);
+    }
+    group_sync<CS>();
   }
 }
 

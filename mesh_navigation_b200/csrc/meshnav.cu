@@ -4,7 +4,9 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <functional>
+#include <map>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -95,6 +97,14 @@ struct WaveBuffers {
   DeviceBuffer<GroupCtl> ctl;
 };
 struct DijkstraBatchBuffers { DeviceBuffer<float> label; DeviceBuffer<uint32_t> mark, list0, list1; DeviceBuffer<GroupCtl> ctl; };
+// one resident wave of mnb_cvp_batch_replan: its goal (seed face, seed position bits), whether it holds that goal's wave of
+// the store's costs and cost limit, and its own allocation (ReplanSlot, kernels_wavefront.cuh) -- growing the store moves
+// no slot
+struct BatchReplanSlot {
+  uint32_t face = 0, pos[3] = {0, 0, 0};
+  bool valid = false;
+  DeviceBuffer<uint8_t> mem;
+};
 
 // Everything that is sized by the mesh or computed from it, with the flags and counters that describe it.  A
 // default-constructed value is "no mesh": free_mesh assigns one, so a buffer declared here needs no other bookkeeping.
@@ -141,6 +151,11 @@ struct MeshState : RayCasterState {
   bool rw_valid = false; uint32_t rw_seed_face = 0, rw_seed_pos[3] = {0, 0, 0}; uint64_t rw_cost_limit = 0, rw_cost_gen = 0;
   uint32_t rw_pool_top = 0;
   DeviceBuffer<uint32_t> d_replan_chg, d_replan_t0;      // the changed list of a replan, T0 and the block minima of its reduction
+  // mnb_cvp_batch_replan: the resident slots (at most one per goal), the cost limit and cost generation their waves were
+  // computed for, the goal table and the T0 minima of a call
+  std::vector<BatchReplanSlot> brs;
+  uint64_t brs_cost_limit = 0, brs_cost_gen = 0;
+  DeviceBuffer<BatchReplanGoal> d_brs_goals; DeviceBuffer<uint32_t> d_brs_minima;
   DeviceBuffer<float> d_path_pos; DeviceBuffer<uint32_t> d_path_face; DeviceBuffer<int32_t> d_bt_result;
   DeviceBuffer<uint32_t> d_bt_spill_list, d_bt_spill_key;   // F each: k_backtrack's unbounded face search (first walk that needs it)
   DeviceBuffer<uint8_t> d_infl_invalid;
@@ -189,6 +204,7 @@ struct mnb_ctx : MeshState {
                                         // Chosen per mesh by mnb_set_mesh unless fixed by mnb_debug_set_layers_smem.
   bool layers_explicit = false;
   uint32_t replan_pool_room = 0;   // level-pool words a resumed replan wave may add (mnb_debug_set_replan_pool_room; 0 = the pool's)
+  uint32_t brs_max_slots = 0xffffffffu;   // cap on the resident slots of mnb_cvp_batch_replan (mnb_debug_set_batch_replan_slots)
   int sweeps = -1;             // in-round sweeps of the whole-grid single plans (mnb_debug_set_sweeps); -1 = derived from the band width
   int cvp_epilogue = 0;        // single-plan epilogue (mnb_debug_set_cvp_epilogue): 0 row replay where it applies, 1 CSR replay for all
   float grid_delta = 1.8f;     // band width of the whole-grid single-plan kernel (wide band + in-round sweeps)
@@ -1161,6 +1177,140 @@ static int32_t impl_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* s
   return MNB_SUCCESS;
 }
 
+// mnb_cvp_batch_replan: mnb_cvp_batch_fields' rows for n goals, with the waves of the distinct goals resident in slots
+// keyed by goal (DESIGN §4, "Batch replan").  Slots of goals absent from the call are released; a goal without one gets
+// one while the cap and the device memory left after the workspace allow it.  A slot's wave resumes from its T0 when it
+// holds the goal's wave of the same cost limit and cost generation (k_batch_replan_t0 decides the rest on the device).
+static int32_t impl_cvp_batch_replan(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
+                                     uint32_t n_changed, const uint32_t* changed, float* out_dist, uint32_t* out_pred, float* out_dir,
+                                     int32_t* out_cut) {
+  if (!ctx || !seed_faces || !seed_pos || (!out_dist && !out_pred && !out_dir && !out_cut) || !ctx->V || n == 0 || (n_changed && !changed))
+    return MNB_E_ARG;
+  const RepairRequest rq{n_changed, changed};
+  int32_t rc;
+  if ((rc = check_changed(ctx, &rq)) != MNB_OK) return rc;
+  if (!ctx->costs_set) { ctx->err = "costs not set"; return MNB_E_STATE; }
+  for (uint32_t i = 0; i < n; ++i) if (seed_faces[i] >= ctx->F) return MNB_INVALID_START;
+  CK(cudaSetDevice(ctx->device));
+  const uint32_t V = ctx->V, pool_cap = ws_pool_cap(V);
+  const size_t slot_bytes = replan_slot_bytes(V, pool_cap);
+  // the distinct goals in the order of their first row; key = seed face and the bits of the seed position
+  using Key = std::array<uint32_t, 4>;
+  std::map<Key, uint32_t> goal_index;
+  std::vector<Key> keys; std::vector<uint32_t> goal_of(n), first;
+  for (uint32_t i = 0; i < n; ++i) {
+    Key k{seed_faces[i], 0, 0, 0};
+    std::memcpy(&k[1], seed_pos + 3 * (size_t)i, 3 * sizeof(float));
+    const auto it = goal_index.emplace(k, (uint32_t)keys.size());
+    if (it.second) { keys.push_back(k); first.push_back(i); }
+    goal_of[i] = it.first->second;
+  }
+  const uint32_t U = (uint32_t)keys.size();
+  std::vector<uint32_t> u_faces(U); std::vector<float> u_pos(3 * (size_t)U);
+  for (uint32_t u = 0; u < U; ++u) {
+    u_faces[u] = seed_faces[first[u]];
+    std::copy(seed_pos + 3 * (size_t)first[u], seed_pos + 3 * (size_t)first[u] + 3, &u_pos[3 * (size_t)u]);
+  }
+  uint64_t limit_bits;
+  std::memcpy(&limit_bits, &cost_limit, sizeof(limit_bits));
+  // release the slots of absent goals and those past the cap; other costs: the waves are stale
+  std::vector<BatchReplanSlot>& slots = ctx->brs;
+  const auto key_of = [](const BatchReplanSlot& s) { return Key{s.face, s.pos[0], s.pos[1], s.pos[2]}; };
+  slots.erase(std::remove_if(slots.begin(), slots.end(), [&](const BatchReplanSlot& s) { return !goal_index.count(key_of(s)); }), slots.end());
+  if (slots.size() > ctx->brs_max_slots) slots.resize(ctx->brs_max_slots);
+  if (ctx->brs_cost_limit != limit_bits || ctx->brs_cost_gen != ctx->cost_gen)
+    for (auto& sl : slots) sl.valid = false;
+  std::vector<int64_t> slot_of(U, -1);
+  for (size_t k = 0; k < slots.size(); ++k) slot_of[goal_index[key_of(slots[k])]] = (int64_t)k;
+  if ((rc = ensure_seeds(ctx, U)) != MNB_OK) return rc;
+  CallerArrays io(ctx);
+  const size_t rows = (size_t)n * V;
+  float* const o_dist = io.out(out_dist, ctx->d_out_dist, rows);
+  uint32_t* const o_pred = io.out(out_pred, ctx->d_batch_pred, rows);
+  float* const o_dir = io.out(out_dir, ctx->d_batch_dir, rows);
+  int32_t* const o_cut = io.out(out_cut, ctx->d_batch_cut, rows);
+  CK(io.status());
+  CvpBatchReplanArgs a{};
+  unsigned launches = 1;
+  auto prepare = [&](unsigned groups) -> int32_t {
+    int32_t r;
+    if ((r = ensure_workspace(ctx, groups)) != MNB_OK) return r;
+    // new slots: as many as the device memory left after the workspace allows, less the reserve batch_shape keeps
+    size_t free_b = 0, total_b = 0;
+    CK(device_memory(ctx->device, &free_b, &total_b));
+    const size_t reserve = std::max<size_t>((size_t)512 << 20, total_b / 32);
+    size_t room = free_b > reserve ? (free_b - reserve) / slot_bytes : 0;
+    for (uint32_t u = 0; u < U && room > 0 && slots.size() < ctx->brs_max_slots; ++u) {
+      if (slot_of[u] >= 0) continue;
+      BatchReplanSlot sl;
+      if (sl.mem.reserve(slot_bytes) != cudaSuccess) { (void)cudaGetLastError(); break; }
+      sl.face = keys[u][0]; std::copy(&keys[u][1], &keys[u][1] + 3, sl.pos);
+      slot_of[u] = (int64_t)slots.size();
+      slots.push_back(std::move(sl));
+      --room;
+    }
+    std::vector<BatchReplanGoal> table(U);
+    bool any_resume = false;
+    for (uint32_t u = 0; u < U; ++u) {
+      BatchReplanGoal& t = table[u];
+      t = BatchReplanGoal{};
+      t.row = first[u];
+      if (slot_of[u] >= 0) {
+        const BatchReplanSlot& sl = slots[(size_t)slot_of[u]];
+        t.slot = sl.mem.p;
+        t.resume = sl.valid ? 1u : 0u;
+        any_resume = any_resume || sl.valid;
+      }
+    }
+    for (auto& sl : slots) sl.valid = false;     // until this call has succeeded
+    CK(ctx->d_brs_goals.reserve(U));
+    CK(cudaMemcpyAsync(ctx->d_brs_goals, table.data(), sizeof(BatchReplanGoal) * U, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_seed_faces, u_faces.data(), sizeof(uint32_t) * U, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_seed_pos, u_pos.data(), 3 * sizeof(float) * U, cudaMemcpyHostToDevice, ctx->stream));
+    if (any_resume) {
+      // T0 of the goals that may resume: chunks of the changed list per goal, about two blocks per SM in all
+      const uint32_t chunks = std::max(1u, std::min((n_changed + 255u) / 256u, std::max(1u, 2u * (unsigned)ctx->sm_count / U)));
+      CK(ctx->d_replan_chg.reserve(std::max(1u, n_changed))); CK(ctx->d_brs_minima.reserve(6 * (size_t)U * chunks));
+      if (n_changed) CK(cudaMemcpyAsync(ctx->d_replan_chg, changed, sizeof(uint32_t) * n_changed, cudaMemcpyHostToDevice, ctx->stream));
+      BatchReplanT0Args t{};
+      t.V = V; t.pool_cap = pool_cap; t.faces = ctx->d_faces; t.cor_ptr = ctx->d_cor_ptr; t.cor_idx = ctx->d_cor_idx;
+      t.goals = ctx->d_brs_goals; t.seed_faces = ctx->d_seed_faces; t.changed = ctx->d_replan_chg; t.n_changed = n_changed;
+      t.chunks = chunks; t.minima = ctx->d_brs_minima;
+      MNB_LAUNCH(k_batch_replan_t0, (size_t)U * chunks, 256, 0, ctx->stream, t);
+      CK(cudaGetLastError());
+      launches++;
+    }
+    if (ctx->h_cancel) *ctx->h_cancel = 0;
+    ctx->infl_labels_valid = false;            // the wavefront workspace is shared with the inflation wave
+    CK(cudaMemsetAsync(ctx->d_next_query, 0, sizeof(unsigned int), ctx->stream));
+    CK(cudaMemsetAsync(ctx->ws.ctl, 0, sizeof(GroupCtl) * groups, ctx->stream));
+    fill_cvp_args(ctx, a);
+    a.n_queries = U; a.robot_face = -1; a.cost_limit = cost_limit; a.goal_dist_offset = 0.0;
+    a.out_dist = o_dist; a.out_pred = o_pred; a.out_dir = o_dir; a.out_cut = o_cut;
+    a.goals = ctx->d_brs_goals; a.pool_room = ctx->replan_pool_room;
+    return MNB_OK;
+  };
+  unsigned groups = 1;
+  rc = run_batch(ctx, [](auto c) { return k_cvp_batch_replan<decltype(c)::value>; }, a, U, ws_bytes_per_group(V), ctx->ws_groups, "CVP",
+                 prepare, &groups);
+  if (rc != MNB_OK) return rc;
+  // duplicate goals: copies of their first row
+  for (uint32_t i = 0; i < n; ++i) {
+    const size_t src = (size_t)first[goal_of[i]] * V, dst = (size_t)i * V;
+    if (src == dst) continue;
+    if (o_dist) CK(cudaMemcpyAsync(o_dist + dst, o_dist + src, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (o_pred) CK(cudaMemcpyAsync(o_pred + dst, o_pred + src, sizeof(uint32_t) * V, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (o_dir) CK(cudaMemcpyAsync(o_dir + dst, o_dir + src, sizeof(float) * V, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (o_cut) CK(cudaMemcpyAsync(o_cut + dst, o_cut + src, sizeof(int32_t) * V, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  CK(io.copy_back());
+  if ((rc = finish_stats(ctx, groups, launches)) != MNB_OK) return rc;
+  if (ctx->h_cancel && *ctx->h_cancel) return MNB_CANCELED;
+  for (auto& sl : slots) sl.valid = true;
+  ctx->brs_cost_limit = limit_bits; ctx->brs_cost_gen = ctx->cost_gen;
+  return MNB_SUCCESS;
+}
+
 static int32_t impl_dijkstra(mnb_ctx* ctx, uint32_t seed_vertex, int64_t robot_vertex, double cost_limit, double goal_dist_offset,
                      float* out_dist, uint32_t* out_pred) {
   if (!ctx || !ctx->V) return MNB_E_ARG;
@@ -1447,6 +1597,20 @@ int32_t mnb_debug_set_sweep_slots(mnb_ctx* ctx, int32_t n) {
 // test hook (not part of the public header): a resumed replan wave may add at most `words` level-pool words (0 = no limit
 // but the pool's), so that tests reach the whole-wave retry after a resumed wave ran out of pool
 int32_t mnb_debug_set_replan_pool_room(mnb_ctx* ctx, uint32_t words) { if (!ctx) return MNB_E_ARG; ctx->replan_pool_room = words; return MNB_OK; }
+// the most resident slots mnb_cvp_batch_replan keeps (n < 0: no cap but the device memory); slots past it are released by
+// the next call
+int32_t mnb_debug_set_batch_replan_slots(mnb_ctx* ctx, int32_t n) {
+  if (!ctx) return MNB_E_ARG;
+  ctx->brs_max_slots = n < 0 ? 0xffffffffu : (uint32_t)n;
+  return MNB_OK;
+}
+// the resident slots of mnb_cvp_batch_replan and how many of them hold a wave the next call may resume
+int32_t mnb_debug_get_batch_replan_slots(mnb_ctx* ctx, uint32_t* n_slots, uint32_t* n_valid) {
+  if (!ctx || !n_slots || !n_valid) return MNB_E_ARG;
+  *n_slots = (uint32_t)ctx->brs.size();
+  *n_valid = (uint32_t)std::count_if(ctx->brs.begin(), ctx->brs.end(), [](const BatchReplanSlot& s) { return s.valid; });
+  return MNB_OK;
+}
 
 int32_t mnb_debug_set_infl_skip(mnb_ctx* ctx, int32_t on) { if (!ctx) return MNB_E_ARG; ctx->infl_skip_clean = on != 0; return MNB_OK; }
 int32_t mnb_debug_set_layers_smem(mnb_ctx* ctx, int32_t mode) {
@@ -1864,6 +2028,19 @@ int32_t mnb_cvp_batch_fields(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_face
   return guarded(ctx, [&]() {
     return impl_cvp_batch_fields(ctx, n, seed_faces, seed_pos, cost_limit, out_dist, out_pred, out_direction, out_cutting_face);
   });
+}
+int32_t mnb_cvp_batch_replan(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
+                             uint32_t n_changed, const uint32_t* changed, float* out_dist, uint32_t* out_pred, float* out_direction,
+                             int32_t* out_cutting_face) {
+  return guarded(ctx, [&]() {
+    return impl_cvp_batch_replan(ctx, n, seed_faces, seed_pos, cost_limit, n_changed, changed, out_dist, out_pred, out_direction, out_cutting_face);
+  });
+}
+int32_t mnb_cvp_batch_replan_release(mnb_ctx* ctx) {
+  if (!ctx) return MNB_E_ARG;
+  CK(cudaSetDevice(ctx->device));
+  ctx->brs.clear();
+  return MNB_OK;
 }
 int32_t mnb_cvp_batch(mnb_ctx* ctx, uint32_t n, const uint32_t* seed_faces, const float* seed_pos, double cost_limit,
                       float* out_dist) {
